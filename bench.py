@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- flow-rows/s classified per model on B200 (BASELINE.json metric), one JSON line on stdout.
+"""bench.py -- flow-rows/s classified per model on H100, one JSON line on stdout.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--workload gnb|logistic|kmeans|forest|forest_hbm|knn|svc]
-                    [--impl reference] [--no-extras]
+                    [--impl reference] [--no-extras] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
            bench.py --gpus N --steps K --warmup W
 
@@ -13,7 +13,12 @@ float32 and already resident in HBM for `value`; `e2e` goes through the public e
 buffers (H2D rows + D2H labels inside the timed region).  The other models/configs are measured in the same run
 and reported under "models" (each with its own roofline and e2e), so the single line carries every model.
 `cpu_baseline` / `--impl reference` time scikit-learn -- the library whose predict() the reference calls at
-traffic_classifier.py:106 -- on the box's host cores.
+traffic_classifier.py:106 -- on the host cores.
+`--dump-outputs DIR` writes, after the timed steps, the labels (class indices) the timed path computed in its last step
+as DIR/<workload>.labels.npy (float32; workloads of more than 1M rows: a fixed sample of 1M rows, every (n // 1M)-th row
+from an offset drawn with seed n).  Inputs are seeded, so two builds can be compared output for output; nine workloads
+write 36 MB.  `--steps K` / `--warmup W` apply to every workload of the line (device-resident steps and the end-to-end
+calls alike); each model entry reports the counts it used.
 """
 from __future__ import annotations
 
@@ -30,7 +35,8 @@ import numpy as np
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
-L2_BYTES = 126 << 20
+L2_BYTES = 50 << 20                 # H100 SXM
+DUMP_ROWS = 1_000_000               # --dump-outputs: rows per workload (a seeded sample beyond this)
 # the arithmetic each kernel computes in (a description, not a precision claim: labels are the fp64 definition's everywhere)
 DTYPES = {"gnb": "f32 certified pre-pass + f64 re-evaluation of uncertified rows", "linear": "f64", "kmeans": "f64",
           "forest": "f32 compares (exact) + f64 accumulation", "knn": "bf16x3 tensor-core filter + f64 exact re-evaluation",
@@ -103,15 +109,14 @@ def _build_workload(name, quick=False):
     if name == "forest_hbm":
         spec = synth.random_forest_spec(n_trees=100, depth=16, seed=seed + 5, full=True)
         return dict(spec=spec, sk=None, d=12, rows=2_000_000 if not quick else 200_000, bytes_per_row=52, flops_per_row=0,
-                    desc="adversarial forest: 100 complete depth-16 trees (13.1M nodes, 105 MB: L2-resident), 2M rows",
+                    desc="adversarial forest: 100 complete depth-16 trees (13.1M nodes, 105 MB), 2M rows",
                     bound="hbm", cpu_sample_rows=100_000, visits_per_row=100 * 17.0)
     if name == "forest_hbm2":
-        # the regime the "fraction of HBM peak" target is about: the node array (268 MB) does not fit the 126 MB L2
-        # (uniform thresholds and uniform rows: every leaf is reached, the walk's working set is the whole array; with
-        # flow-shaped rows the same forest is touched on 58 MB only -- ncu r02 -- and stays in L2)
+        # the node array (268 MB) does not fit the 50 MB L2, and uniform thresholds with uniform rows reach every leaf:
+        # the walk's working set is the whole array
         spec = synth.random_forest_spec(n_trees=256 if not quick else 32, depth=16, seed=seed + 6, full=True, uniform=True)
         return dict(spec=spec, sk=None, d=12, rows=1_000_000 if not quick else 100_000, bytes_per_row=52, flops_per_row=0,
-                    desc="adversarial forest, HBM-resident: 256 complete depth-16 trees (33.6M nodes, 268 MB > 126 MB L2), uniform "
+                    desc="adversarial forest, HBM-resident: 256 complete depth-16 trees (33.6M nodes, 268 MB > 50 MB L2), uniform "
                          "thresholds, 1M rows uniform in [0,1)^12 (every leaf reached)",
                     bound="hbm", cpu_sample_rows=20_000, visits_per_row=256 * 17.0, rows_kind="uniform")
     if name == "knn":
@@ -218,27 +223,27 @@ class ClockSampler:
 
 # ----------------------------------------------------------------------------- measurement
 def ring_size(rows, row_bytes):
-    """distinct batches the timed steps rotate through, so that consecutive steps never find their rows in the 126 MiB L2"""
+    """distinct batches the timed steps rotate through, so that consecutive steps never find their rows in the 50 MiB L2"""
     if rows * row_bytes >= L2_BYTES * 1.25:
         return 1
     return min(12, max(2, int(np.ceil((L2_BYTES * 1.25) / (rows * row_bytes))) + 1))
 
 
 def make_config(w, world):
-    """the `config` object, identical in the b200 and the reference arm (it describes the workload, not the implementation)"""
+    """the `config` object, identical in the GPU and the reference arm (it describes the workload, not the implementation)"""
     ring = ring_size(w["rows"], 4 * w["d"])
     return {"workload": w["desc"], "rows_per_gpu_per_step": w["rows"], "n_features": w["d"],
             "input": "float32 rows: resident in HBM for `value`, in page-locked host memory for `e2e`",
             "parallelism": f"row-sharded x{world}: every rank classifies its own rows with its own model replica, no collective on the "
                            "data path; `value_with_gather` adds the one all-gather of per-shard label vectors (uint8 on the wire)",
-            "l2": (f"{ring} distinct batches rotate ({ring * w['rows'] * 4 * w['d'] >> 20} MiB > 126 MiB L2)" if ring > 1 else
-                   f"one batch of {w['rows'] * 4 * w['d'] >> 20} MiB > 126 MiB L2")}
+            "l2": (f"{ring} distinct batches rotate ({ring * w['rows'] * 4 * w['d'] >> 20} MiB > 50 MiB L2)" if ring > 1 else
+                   f"one batch of {w['rows'] * 4 * w['d'] >> 20} MiB > 50 MiB L2")}
 
 
 def bind_to_gpu_numa_node(index):
     """Pin this process (and so its page-locked staging buffers, first touch) to the NUMA node the GPU hangs off: with
     eight ranks streaming host rows at once, buffers on the far socket cross the inter-socket link and the root complexes
-    contend (e2e efficiency 0.81 at N = 8 in round 1).  Returns a short description; silently does nothing when the
+    contend.  Returns a short description; silently does nothing when the
     topology is not exposed (containers, single-node hosts)."""
     try:
         import torch
@@ -286,7 +291,7 @@ def max_over_ranks(x, world, device):
     return float(t.item())
 
 
-def measure_with_gather(w, steps, world, device):
+def measure_with_gather(w, steps, warmup, world, device):
     """SURVEY 8(e): the N-GPU step WITH the one collective of the path -- every rank classifies its block, then ONE all-gather
     of the per-shard label vectors puts the full vector on every rank (tcsdn_allgather_labels_u8: class indices travel as
     bytes).  predict + gather are enqueued on one stream with no host synchronisation and the K steps are captured into
@@ -305,7 +310,7 @@ def measure_with_gather(w, steps, world, device):
     side = torch.cuda.Stream(device=device)
     side.wait_stream(torch.cuda.current_stream())
     with torch.cuda.stream(side):
-        for _ in range(3):                       # warm-up outside the capture (also sizes the communicator's staging buffer)
+        for _ in range(warmup):                  # warm-up outside the capture (also sizes the communicator's staging buffer)
             est.predict_indices(x, out=lab)
             comm.allgather_labels(lab, rows, n_classes=n_classes, out=allv)
     torch.cuda.synchronize()
@@ -347,7 +352,7 @@ def measure_with_gather(w, steps, world, device):
     try:
         comm.gather_buffer(rows)
         with torch.cuda.stream(side):
-            for _ in range(3):
+            for _ in range(warmup):
                 got = comm.predict_gathered(est, x)
         torch.cuda.synchronize()
         barrier(world)
@@ -394,7 +399,7 @@ def measure_gpu(w, steps, warmup, world, device, peaks, extras_light=False, cloc
     import torch
     from traffic_classifier_sdn_b200 import from_spec
     est = from_spec(w["spec"])
-    for key, val in OPTIONS:          # --set-option K=V (tuning sweeps; defaults are the measured best)
+    for key, val in OPTIONS:          # --set-option K=V (tuning sweeps)
         est.set_option(key, val)
     rows, d = w["rows"], w["d"]
     row_bytes = 4 * d
@@ -467,7 +472,7 @@ def measure_gpu(w, steps, warmup, world, device, peaks, extras_light=False, cloc
     # Three variants: rows in page-locked memory (the headline `value`), the same through predict_indices with a
     # page-locked int32 result buffer (no label materialisation: what a pipeline that keeps indices would see), and
     # rows in ordinary pageable memory.
-    e2e_steps = max(3, min(steps, 10)) if not extras_light else 3
+    e2e_steps = steps
     host = [torch.empty((rows, d), dtype=torch.float32).pin_memory() for _ in range(min(ring, 3))]
     for h, b in zip(host, batches):
         h.copy_(b)
@@ -488,7 +493,7 @@ def measure_gpu(w, steps, warmup, world, device, peaks, extras_light=False, cloc
     e2e_predict = timed(lambda i: est.predict(host_np[i % len(host_np)]), e2e_steps)
     e2e_indices = timed(lambda i: est.predict_indices(host_np[i % len(host_np)], out=lab_host), e2e_steps)
     pageable = np.array(host_np[0], copy=True)                            # ordinary (pageable) memory
-    e2e_pageable = timed(lambda i: est.predict(pageable), max(2, e2e_steps // 2))
+    e2e_pageable = timed(lambda i: est.predict(pageable), e2e_steps)
     del pageable
     e2e = e2e_predict
 
@@ -529,23 +534,17 @@ def measure_gpu(w, steps, warmup, world, device, peaks, extras_light=False, cloc
             del gcopy, src, dst
         except Exception as exc:
             copy_at_size = {"error": f"{type(exc).__name__}: {exc}"}
-    tr = load_traffic(w["name"])
-    if tr is not None:
-        # the capture was taken on the full-size workload; scale if this run uses another batch size (--quick)
-        tr = dict(tr, bytes=tr["bytes"] * rows / w["full_rows"])
-    roofline = dict(bound=w["bound"], achieved=achieved, peak=peak, unit=unit, frac=achieved / peak,
-                    traffic=None if tr is None else tr["bytes"], traffic_source=None if tr is None else tr["source"],
-                    peak_source=peaks["source"])
+    roofline = dict(bound=w["bound"], achieved=achieved, peak=peak, unit=unit, frac=achieved / peak, peak_source=peaks["source"])
     if copy_at_size is not None:
         roofline["copy_at_this_size"] = copy_at_size
         if "gbs" in copy_at_size:
             roofline["frac_of_copy_at_this_size"] = achieved / copy_at_size["gbs"]
     if w["bound"] == "tensor":
         # SURVEY 8(d): next to the algorithmic flops, the flops the tensor cores are actually ISSUED (bf16 x 3 split:
-        # K = 80 per pair instead of d = 12, reference rows padded to 64-row tiles) and the ncu tensor-pipe figure
+        # K = 80 per pair instead of d = 12, reference rows padded to 64-row tiles)
         issued_per_row = w["issued_mma_flops_per_row"]
         if w["name"] == "knn":
-            # the engine leaves out the reference tiles that are too far for all 512 rows of a pass (exact: DESIGN 4): what the
+            # the engine leaves out the reference tiles that are too far for all 256 rows of a pass (exact: DESIGN 4): what the
             # tensor cores are issued is the tiles actually multiplied (the engine's own counter), `achieved` stays the
             # brute-force-equivalent rate (every pair counted, as sklearn's brute force computes them)
             st = est.stats()
@@ -556,21 +555,21 @@ def measure_gpu(w, steps, warmup, world, device, peaks, extras_light=False, cloc
                             achieved_is="brute-force-equivalent flops (all 10M x 50k pairs) per second; issued_mma counts the tiles actually multiplied",
                             tie_rows_rerun_in_index_order=int(st[7]))
         issued = rows * issued_per_row / (kernel_ms * 1e-3) / 1e12
-        roofline.update(issued_mma=issued, issued_mma_frac=issued / peak, tensor_pipe_pct_ncu=load_summary_field(w["name"], "tensor_pipe_pct"))
+        roofline.update(issued_mma=issued, issued_mma_frac=issued / peak)
         if w.get("exp_per_row"):
             # SVC is bound by the MUFU unit, not the tensor pipe (SURVEY 8d): one ex2 per (row, support vector) pair against
-            # 16 lanes/clk/SM (measured, tools/tmem_probe.cu) x 148 SMs x the SM clock
+            # 16 results/clk/SM (CUDA C programming guide, compute capability 9.0) x the SMs x the SM clock
             exp_s = rows * w["exp_per_row"] / (kernel_ms * 1e-3)
-            exp_peak = 16.0 * 148 * (peaks.get("sm_max_mhz") or 1965.0) * 1e6
-            roofline.update(exp_per_s=exp_s, exp_peak=exp_peak, exp_frac=exp_s / exp_peak, xu_pipe_pct_ncu=load_summary_field(w["name"], "xu_pipe_pct"))
-    return dict(value=value, ms_per_step=ms / steps, kernel_ms=kernel_ms, rows=rows, ring=ring, mode=mode, traffic=tr,
+            exp_peak = 16.0 * torch.cuda.get_device_properties(device).multi_processor_count * (peaks.get("sm_max_mhz") or 1980.0) * 1e6
+            roofline.update(exp_per_s=exp_s, exp_peak=exp_peak, exp_frac=exp_s / exp_peak)
+    return dict(value=value, ms_per_step=ms / steps, kernel_ms=kernel_ms, rows=rows, ring=ring, mode=mode, steps=steps, warmup=warmup,
                 launches_per_step=launches_per_step, load_window=load_window,
-                e2e=dict(value=e2e, unit="flow-rows/s", h2d_bytes_per_step=rows * row_bytes, d2h_bytes_per_step=rows * 4,
+                e2e=dict(value=e2e, unit="flow-rows/s", steps=e2e_steps, h2d_bytes_per_step=rows * row_bytes, d2h_bytes_per_step=rows * 4,
                          call="estimator.predict(X): float32 rows in page-locked host memory -> numpy labels (classes_.take included)",
                          indices_value=e2e_indices, indices_call="estimator.predict_indices(X, out=page-locked int32): no label materialisation",
                          pageable_value=e2e_pageable, pageable_call="estimator.predict(X) on rows in pageable host memory",
                          bound="PCIe: host rows cross at ~48-55 GB/s per GPU; the streaming models' kernels are 50-100x faster than the copy"),
-                roofline=roofline, est=est, batch0=batches[0])
+                roofline=roofline, est=est, batch0=batches[0], labels=lab_dev)
 
 
 def _threadpools():
@@ -709,39 +708,28 @@ def per_row_call_pattern(w, est, seconds=1.0):
     return out
 
 
-def load_traffic(name):
-    """DRAM bytes per launch of the workload's dominant kernel, from the committed ncu capture (profiles/)."""
-    best = None
-    pdir = os.path.join(ROOT, "profiles")
-    if os.path.isdir(pdir):
-        for f in sorted(os.listdir(pdir)):
-            if f.endswith("_ncu_summary.json"):
-                j = json.load(open(os.path.join(pdir, f)))
-                if name in j and j[name].get("dram_bytes"):
-                    best = {"bytes": j[name]["dram_bytes"], "source": f"profiles/{f}"}
-    return best
-
-
-def load_summary_field(name, field):
-    """Latest committed ncu summary's value of `field` for the workload (profiles/*_ncu_summary.json), or None."""
-    best = None
-    pdir = os.path.join(ROOT, "profiles")
-    if os.path.isdir(pdir):
-        for f in sorted(os.listdir(pdir)):
-            if f.endswith("_ncu_summary.json"):
-                j = json.load(open(os.path.join(pdir, f)))
-                if name in j and j[name].get(field) is not None:
-                    best = j[name][field]
-    return best
-
-
 def load_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         j = json.load(open(p))
-        return dict(hbm_gbs=float(j["hbm_gbs"]), bf16_tflops=float(j.get("bf16_tflops", 1590.0)), sm_max_mhz=float(j.get("sm_max_mhz", 1965.0)),
+        return dict(hbm_gbs=float(j["hbm_gbs"]), bf16_tflops=float(j.get("bf16_tflops", 989.0)), sm_max_mhz=float(j.get("sm_max_mhz", 1980.0)),
                     source="measured")
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, source="fallback")
+    # NVIDIA's H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, source="data sheet")
+
+
+def dump_outputs(out_dir, name, labels):
+    """the labels of the last timed step as out_dir/<name>.labels.npy (float32); beyond DUMP_ROWS rows a strided sample
+    whose row indices depend only on the row count (offset seeded with it)"""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    n = labels.numel()
+    if n > DUMP_ROWS:
+        stride = n // DUMP_ROWS
+        offset = int(torch.randint(0, stride, (1,), generator=torch.Generator().manual_seed(n)))
+        rows = offset + stride * torch.arange(DUMP_ROWS, device=labels.device)
+        labels = labels[rows]
+    np.save(os.path.join(out_dir, f"{name}.labels.npy"), labels.cpu().numpy().astype(np.float32))
 
 
 def main():
@@ -757,6 +745,8 @@ def main():
     ap.add_argument("--gpu-only", action="store_true", help="skip the scikit-learn baselines (tuning sweeps)")
     ap.add_argument("--set-option", action="append", default=[], metavar="KEY=VALUE",
                     help="tcsdn_set_option on every estimator (include/tcsdn.h TCSDN_OPT_*), e.g. 4=3")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the labels the timed path computed in its last step, per workload, as DIR/<workload>.labels.npy")
     args = ap.parse_args()
     for kv in args.set_option:
         OPTIONS.append((int(kv.split("=")[0]), int(kv.split("=")[1])))
@@ -797,6 +787,8 @@ def main():
     sampler = ClockSampler(local)
     sampler.start()
     head = measure_gpu(w, args.steps, args.warmup, world, device, peaks, clock_probe_s=1.5)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, args.workload, head["labels"])
     clocks = sampler.stop(*head["load_window"])
     clocks["how"] = "nvidia-smi -lms 100 over a 1.5 s continuation of the timed CUDA graph (same kernels, same batches)"
 
@@ -805,10 +797,11 @@ def main():
         for name in [x for x in args.extras.split(",") if x and x != args.workload]:
             try:
                 wx = build_workload(name, args.quick)
-                steps_x = max(3, min(args.steps, 5))
-                r = measure_gpu(wx, steps_x, 3, world, device, peaks, extras_light=True)
+                r = measure_gpu(wx, args.steps, args.warmup, world, device, peaks, extras_light=True)
+                if args.dump_outputs and rank == 0:
+                    dump_outputs(args.dump_outputs, name, r["labels"])
                 entry = {"workload": wx["desc"], "dtype": DTYPES.get(wx["spec"]["kind"]), "value": r["value"], "unit": "flow-rows/s", "rows_per_gpu_per_step": r["rows"],
-                         "ms_per_step": r["ms_per_step"], "e2e": r["e2e"], "roofline": r["roofline"],
+                         "ms_per_step": r["ms_per_step"], "steps": r["steps"], "warmup": r["warmup"], "e2e": r["e2e"], "roofline": r["roofline"],
                          "gpu_launches_per_step": r["launches_per_step"], "engine_stats": r["est"].stats().tolist(),
                          "timed_region": r["mode"]}
                 if rank == 0 and world == 1 and not args.gpu_only:
@@ -829,7 +822,7 @@ def main():
     gathered = None
     if world > 1:
         try:
-            gathered = measure_with_gather(w, args.steps, world, device)
+            gathered = measure_with_gather(w, args.steps, args.warmup, world, device)
         except Exception as exc:   # the headline line must survive a failure of this extra
             gathered = {"error": f"{type(exc).__name__}: {exc}"}
     if rank == 0:

@@ -1,5 +1,5 @@
 /*
- * tcsdn.h -- C ABI of libtcsdn.so: B200 (sm_100a) kernels for the per-flow classification path of
+ * tcsdn.h -- C ABI of libtcsdn.so: H100 (sm_90a) kernels for the per-flow classification path of
  * ashwinn-v/Traffic-classifier-SDN.
  *
  * What this boundary replaces.  The reference has no FFI; its hot path is two Python statements:
@@ -65,7 +65,7 @@ enum { /* tcsdn_set_option() keys */
                                   4 svc engine, tests only: scores_out receives the certificate's per-pair error bounds */
     TCSDN_OPT_CHUNK_ROWS = 2,  /* host-pointer pipeline chunk (rows); 0 = default */
     TCSDN_OPT_CHECK_FINITE = 3, /* 1 (default): fail with TCSDN_ENONFINITE on NaN/inf input */
-    /* measurement knobs (defaults are the measured best; tools/gpu_check.sh sweeps them) */
+    /* measurement knobs (bench.py --set-option sweeps them) */
     TCSDN_OPT_SCORER_SHAPE = 4,    /* streaming scorers' CTA shape: 0 auto, 1 = 128 threads x 4 rows, 2 = 256 x 2, 3 = 128 x 2 */
     TCSDN_OPT_FOREST_SHAPE = 5,    /* forest CTA shape: 0 auto, 1 = 512 threads x 2 rows, 2 = 256 x 4, 3 = 1024 x 1 */
     TCSDN_OPT_FOREST_SORT = 6,     /* 1 (default): re-assign a tile's rows to threads in tree-0 leaf order */

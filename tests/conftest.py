@@ -1,3 +1,4 @@
+import glob
 import os
 import sys
 
@@ -13,15 +14,23 @@ KINDS = ("linear", "gnb", "kmeans", "knn", "svc", "forest")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
+
+
+def load_golden():
+    """tests/golden/bundled.*.npz, merged: the reference's bundled rows, its six models' parameters and
+    scikit-learn's answers (made by tests/golden/make_golden.py, split into parts below 1 MB)."""
+    g = {}
+    for path in sorted(glob.glob(os.path.join(ROOT, "tests", "golden", "bundled.*.npz"))):
+        z = np.load(path, allow_pickle=False)
+        g.update({k: z[k] for k in z.files})
+    assert "X" in g, "tests/golden/bundled.*.npz missing"
+    return g
 
 
 @pytest.fixture(scope="session")
 def golden():
-    """tests/golden/bundled.npz: the reference's bundled rows, its six models' parameters and
-    scikit-learn's answers (made by tests/golden/make_golden.py in the build container)."""
-    z = np.load(os.path.join(ROOT, "tests", "golden", "bundled.npz"), allow_pickle=False)
-    return {k: z[k] for k in z.files}
+    return load_golden()
 
 
 def spec_from_golden(g, kind):

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Generate tests/golden/bundled.npz from the reference tree (run in the build container only).
+"""Generate tests/golden/bundled.*.npz and tests/golden/datasets/ from the reference tree.
 
-    python tests/golden/make_golden.py [/root/reference]
+    python tests/golden/make_golden.py REFERENCE_DIR
 
 Inputs (read-only): the reference's five ``datasets/*_training_data.csv`` and its six
 ``models/*`` pickles.  The rows are assembled with the notebooks' recipe (SURVEY.md 8c:
@@ -11,8 +11,12 @@ cumulative counters).  Expected outputs come from scikit-learn itself -- the lib
 revived from the pickles: the four that still unpickle are loaded with ``pickle.load`` and
 must agree exactly with their rebuilt twins; KNeighbors / RandomForestClassifier are rebuilt
 from the data-only spec (tests/sk_rebuild.py).  Nothing under /root/reference is copied as
-source; the .npz holds numeric rows, fitted parameters and sklearn's answers.
+source; the .npz files hold numeric rows, fitted parameters and sklearn's answers, split into parts of
+less than 1 MB each (tests/conftest.py load_golden() merges them).  datasets/ holds the first and last
+lines of each training file, so that the recipe test (tests/test_dataio.py) runs on the notebooks' own
+text, together with the positions of those rows in the golden rows.
 """
+import io
 import os
 import pickle
 import sys
@@ -29,6 +33,50 @@ from traffic_classifier_sdn_b200 import modelio  # noqa: E402
 from sk_rebuild import sklearn_from_spec  # noqa: E402
 
 DROP = ["Forward Packets", "Forward Bytes", "Reverse Packets", "Reverse Bytes"]
+PART_BYTES = 900_000          # compressed size of one golden part (every file stays below 1 MB)
+SAMPLE_HEAD, SAMPLE_TAIL = 40, 8   # data lines kept from the start and the end of each training file
+
+
+def save_parts(out):
+    """Greedy split of `out` into tests/golden/bundled.<i>.npz, each at most PART_BYTES compressed."""
+    def size(a):
+        b = io.BytesIO()
+        np.savez_compressed(b, a=a)
+        return len(b.getvalue())
+    parts, cur, cur_bytes = [], {}, 0
+    for k in sorted(out, key=lambda k: -size(out[k])):
+        n = size(out[k])
+        assert n <= PART_BYTES, k
+        if cur and cur_bytes + n > PART_BYTES:
+            parts.append(cur)
+            cur, cur_bytes = {}, 0
+        cur[k] = out[k]
+        cur_bytes += n
+    parts.append(cur)
+    for i, part in enumerate(parts):
+        path = os.path.join(HERE, f"bundled.{i}.npz")
+        np.savez_compressed(path, **part)
+        print("wrote", path, os.path.getsize(path), "bytes")
+
+
+def save_dataset_samples(ref):
+    """Head and tail of every training file (as text), and where their rows sit in the golden rows."""
+    os.makedirs(os.path.join(HERE, "datasets"), exist_ok=True)
+    rows, offset = [], 0
+    for name, sep in (("ping", "\t"), ("voice", "\t"), ("dns", "\t"), ("telnet", "\t"), ("game", ",")):
+        src = os.path.join(ref, "datasets", f"{name}_training_data.csv")
+        with open(src, "rb") as fh:
+            lines = fh.read().split(b"\n")
+        tail_nl = lines[-1] == b""          # a file that ends in a newline splits into a last empty piece
+        data = lines[1:-1] if tail_nl else lines[1:]
+        keep = list(range(SAMPLE_HEAD)) + list(range(len(data) - SAMPLE_TAIL, len(data)))
+        with open(os.path.join(HERE, "datasets", f"{name}_training_data.csv"), "wb") as fh:
+            fh.write(b"\n".join([lines[0]] + [data[i] for i in keep]) + (b"\n" if tail_nl else b""))
+        n_rows = len(pd.read_csv(src, delimiter=sep).dropna())
+        complete = len(pd.read_csv(src, delimiter=sep)) == n_rows   # only a truncated last line is dropped
+        rows += [offset + i for i in keep if complete or i < len(data) - 1]
+        offset += n_rows
+    np.save(os.path.join(HERE, "datasets", "rows.npy"), np.asarray(rows, np.int32))
 
 
 def load_bundled_rows(ref):
@@ -43,7 +91,7 @@ def load_bundled_rows(ref):
 
 
 def main():
-    ref = sys.argv[1] if len(sys.argv) > 1 else "/root/reference"
+    ref = sys.argv[1]
     warnings.simplefilter("ignore")
     X, y = load_bundled_rows(ref)
     assert X.shape == (7653, 12), X.shape
@@ -107,9 +155,8 @@ def main():
             out["forest.expected_score"] = sk.predict_proba(X)
         agree = float(np.mean(classes[lab] == y)) if kind != "kmeans" else float("nan")
         print(f"{fname}: kind={kind} labels ok, agreement with CSV labels {agree:.4f}")
-    path = os.path.join(HERE, "bundled.npz")
-    np.savez_compressed(path, **out)
-    print("wrote", path, os.path.getsize(path), "bytes")
+    save_parts(out)
+    save_dataset_samples(ref)
 
 
 if __name__ == "__main__":

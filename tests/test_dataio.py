@@ -1,14 +1,15 @@
-"""Training-data reader/writer (SURVEY row N4): format round trip, mixed delimiters, truncated tail, and -- where the
-reference checkout is present (this container, not the GPU box) -- the notebooks' 7 653-row recipe against the golden rows."""
+"""Training-data reader/writer (SURVEY row N4): format round trip, mixed delimiters, truncated tail, and the notebooks'
+recipe on the head and tail of each bundled training file (tests/golden/datasets) against the golden rows."""
 import os
 
 import numpy as np
 import pytest
 
+from conftest import load_golden
 from traffic_classifier_sdn_b200 import dataio, flows
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-REF_DATA = "/root/reference/datasets"
+SAMPLE_DATA = os.path.join(HERE, "golden", "datasets")
 
 
 def _table():
@@ -75,10 +76,12 @@ def test_errors(tmp_path):
         dataio.load_training_set([])
 
 
-@pytest.mark.skipif(not os.path.isdir(REF_DATA), reason="reference checkout not present (GPU box)")
 def test_notebook_recipe_reproduces_the_golden_rows():
-    z = np.load(os.path.join(HERE, "golden", "bundled.npz"))
-    paths = [os.path.join(REF_DATA, f"{k}_training_data.csv") for k in ("ping", "voice", "dns", "telnet", "game")]
+    """the first and last lines of the five bundled files (ping's truncated last line included), read with the recipe,
+    give exactly the golden rows at the positions tests/golden/make_golden.py recorded"""
+    z = load_golden()
+    rows = np.load(os.path.join(SAMPLE_DATA, "rows.npy"))
+    paths = [os.path.join(SAMPLE_DATA, f"{k}_training_data.csv") for k in ("ping", "voice", "dns", "telnet", "game")]
     X, y = dataio.load_training_set(paths)
-    assert X.shape == (7653, 12)
-    assert np.array_equal(X, z["X"]) and np.array_equal(y, z["y"].astype(str))
+    assert X.shape == (len(rows), 12) and len(rows) == 5 * 48 - 1
+    assert np.array_equal(X, z["X"][rows]) and np.array_equal(y, z["y"][rows].astype(str))

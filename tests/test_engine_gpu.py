@@ -1,4 +1,4 @@
-"""GPU: the tensor-core (tcgen05) distance engine against the oracle.
+"""GPU: the tensor-core (wgmma) distance engine against the oracle.
 
 KNN through the engine must be bit-identical to the fp64 kernel / oracle / sklearn's sequential heap: the
 tensor-core distances only FILTER candidates, every survivor is re-evaluated in fp64 in index order.

@@ -1,5 +1,5 @@
-"""GPU parity tests (run on the B200 box): the CUDA path, called through the C ABI, against
-  (a) tests/golden/bundled.npz -- sklearn's answers for the reference's six pickles on its bundled rows,
+"""GPU parity tests (run on an H100): the CUDA path, called through the C ABI, against
+  (a) tests/golden/bundled.*.npz -- sklearn's answers for the reference's six pickles on its bundled rows,
   (b) the CPU oracle (oracle/tcsdn_oracle.c) on seeded inputs and edge cases,
   (c) live scikit-learn (installed on the box; the library the reference calls) on fresh fits,
   (d) size-independent properties at BASELINE sizes.

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Run one bench workload a few times on device-resident rows (for ncu): tools/run_workload.py <name> <rows> [reps]"""
+"""Run one bench workload a few times on device-resident rows (for a profiler): tools/run_workload.py <name> <rows> [reps]"""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -1,4 +1,4 @@
-"""traffic_classifier_sdn_b200 -- B200-native (sm_100a) per-flow classification for Traffic-classifier-SDN.
+"""traffic_classifier_sdn_b200 -- H100-native (sm_90a) per-flow classification for Traffic-classifier-SDN.
 
 The package replaces one call of the reference, ``model.predict(rows)`` at ``traffic_classifier.py:106``, for its
 six scikit-learn estimators, with hand-written CUDA kernels behind a C ABI (``include/tcsdn.h``,

@@ -1,4 +1,4 @@
-"""Build libtcsdn.so in-tree with nvcc for sm_100a (B200).  No JIT cache, no torch extension machinery:
+"""Build libtcsdn.so in-tree with nvcc for sm_90a (H100).  No JIT cache, no torch extension machinery:
 the .so sits next to the sources so that it travels to the GPU box with the repository snapshot."""
 import os
 import shutil
@@ -12,7 +12,7 @@ SOURCES = ["abi.cu", "scorers.cu", "forest.cu", "knn.cu", "svc.cu", "flow.cu", "
 # scorers.cu is compiled five times: once as the dispatcher and once per tiled feature count (object name -> extra flags)
 VARIANTS = {"scorers.cu": [("scorers.o", []), ("scorers_d4.o", ["-DTCSDN_SCORER_D=4"]), ("scorers_d8.o", ["-DTCSDN_SCORER_D=8"]),
                            ("scorers_d12.o", ["-DTCSDN_SCORER_D=12"]), ("scorers_d16.o", ["-DTCSDN_SCORER_D=16"])]}
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v"]
 
 
@@ -32,7 +32,7 @@ def needs_build():
 
 
 def build(force=False, verbose=False, extra_flags=(), out=None):
-    """Compile every .cu for sm_100a and link libtcsdn.so.  Returns the library path.
+    """Compile every .cu for sm_90a and link libtcsdn.so.  Returns the library path.
     `extra_flags` / `out`: experiment builds (e.g. -DTCSDN_EXP_NO_EX2) into another file, tools/ only."""
     lib_out = out or LIB
     if not force and not out and not needs_build():
@@ -60,7 +60,7 @@ def build(force=False, verbose=False, extra_flags=(), out=None):
         objs.append(obj)
     with open(os.path.join(objdir, "ptxas.log"), "w") as fh:
         fh.write("\n".join(log))
-    cmd = [nvcc, "-ccbin", "/usr/bin/g++", "-shared", "-o", lib_out] + objs + ["-lcuda", "-ldl"]
+    cmd = [nvcc, "-ccbin", "/usr/bin/g++", "-shared"] + NVCC_FLAGS[:2] + ["-o", lib_out] + objs + ["-lcuda", "-ldl"]
     subprocess.check_call(cmd, env=env)
     if verbose:
         print("\n".join(log))

@@ -34,8 +34,8 @@ static int model_base(tcsdn_model **out, int kind, int d, int n_classes, int sco
     cudaDeviceProp prop;
     e = cudaGetDeviceProperties(&prop, dev);
     if (e != cudaSuccess) { set_error("cudaGetDeviceProperties: %s", cudaGetErrorString(e)); return TCSDN_ECUDA; }
-    if (prop.major < 10) {
-        set_error("device %d is sm_%d%d; libtcsdn is built for sm_100a (B200) only", dev, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) {   // sm_90a code (wgmma) loads on compute capability 9.0 only
+        set_error("device %d is sm_%d%d; libtcsdn is built for sm_90a (H100) only", dev, prop.major, prop.minor);
         return TCSDN_ECUDA;
     }
     tcsdn_model *m = new (std::nothrow) tcsdn_model();
@@ -439,7 +439,7 @@ int tcsdn_predict(tcsdn_model_t *m, const void *x, int64_t n, int32_t d, int32_t
     int64_t chunk = m->opt_chunk_rows;
     if (chunk <= 0) {
         // ~16 MiB of rows per chunk for the streaming kernels (the copy is their bottleneck: small chunks start the overlap early);
-        // 128 MiB for the distance engine, whose persistent CTAs take 512 rows each and want several passes per launch
+        // 128 MiB for the distance engine, whose persistent CTAs take 256 rows per pass and want several passes per launch
         const size_t chunk_bytes = (m->kind == TCSDN_KIND_KNN || m->kind == TCSDN_KIND_SVC) ? (128u << 20) : (16u << 20);
         chunk = (int64_t)(chunk_bytes / row_bytes);
         chunk = (chunk / 1024) * 1024;

@@ -242,18 +242,18 @@ int tcsdn_allgather_labels_u8(tcsdn_comm_t *c, const int32_t *local, int64_t n_l
     uint8_t *mine = c->d_bytes, *gathered = c->d_bytes + c->bytes_cap;
     const int threads = 256;
     int64_t blocks = (nb4 / 4 + threads - 1) / threads;
-    if (blocks > 148 * 8) blocks = 148 * 8;
+    if (blocks > 132 * 8) blocks = 132 * 8;
     labels_pack_u8<<<(unsigned)blocks, threads, 0, st>>>(local, n_local, mine, nb4);
     TCSDN_CUDA(cudaGetLastError());
     TCSDN_NCCL(g_nccl.AllGather(mine, gathered, (size_t)nb4, ncclUint8, c->comm, st));
     if (nb4 == n_block) {
         const int64_t total = n_block * c->world;
         blocks = (total / 4 + threads - 1) / threads;
-        if (blocks > 148 * 8) blocks = 148 * 8;
+        if (blocks > 132 * 8) blocks = 132 * 8;
         labels_unpack_u8<<<(unsigned)blocks, threads, 0, st>>>(gathered, all, total);
     } else {
         for (int r = 0; r < c->world; ++r)   // odd block length: per-rank segments (destination blocks are n_block apart)
-            labels_unpack_u8<<<(unsigned)std::max<int64_t>(1, std::min<int64_t>(blocks, 148 * 8)), threads, 0, st>>>(
+            labels_unpack_u8<<<(unsigned)std::max<int64_t>(1, std::min<int64_t>(blocks, 132 * 8)), threads, 0, st>>>(
                 gathered + (size_t)r * nb4, all + (size_t)r * n_block, n_block);
     }
     TCSDN_CUDA(cudaGetLastError());
@@ -363,7 +363,7 @@ int tcsdn_predict_gathered(tcsdn_model_t *m, tcsdn_comm_t *c, const void *x, int
     peer_barrier_kernel<<<1, 32, 0, st>>>(G, 0);
     if (n_local > 0) {
         int64_t blocks = ((n_local + 15) / 16 + 255) / 256;
-        if (blocks > 148 * 4) blocks = 148 * 4;
+        if (blocks > 132 * 4) blocks = 132 * 4;
         scatter_labels_kernel<<<(unsigned)blocks, 256, 0, st>>>(G, c->d_pad, n_local);
     }
     const int64_t done16 = (n_local + 15) & ~(int64_t)15;

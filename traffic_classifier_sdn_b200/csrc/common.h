@@ -1,4 +1,4 @@
-// common.h -- shared host-side declarations of libtcsdn (B200 / sm_100a only).
+// common.h -- shared host-side declarations of libtcsdn (H100 / sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 
@@ -113,7 +113,7 @@ struct tcsdn_model {
     int dev = 0;
     int n_classes = 0;   // rows of the score matrix for linear/gnb/kmeans; classes for knn/svc/forest
     int score_cols = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     // options
     int64_t opt_engine = 0;
     int64_t opt_chunk_rows = 0;

@@ -1,4 +1,4 @@
-// dist_engine.cu -- tensor-core (tcgen05 / TMEM) distance engine shared by KNeighbors and SVC(rbf).
+// dist_engine.cu -- tensor-core (Hopper wgmma) distance engine shared by KNeighbors and SVC(rbf).
 //
 // Both estimators need, for every (query row x, reference row t) pair, the squared euclidean distance
 //   d(x,t) = ||x||^2 + ||t||^2 - 2 x.t          (reference rows = training rows / support vectors)
@@ -9,7 +9,7 @@
 // Rows are centred on a fixed point of the reference set (distances are translation invariant), rounded to fp32
 // and split into three bf16 pieces h+m+l (8+8+8 mantissa bits: an exact decomposition of the fp32 value).  The
 // products hh, hm, mh, mm, hl, lh are laid side by side along K (6 d slots), three more slots carry the bf16
-// pieces of ||t||^2 against 1.0, and A is pre-scaled by -2, so that ONE tcgen05.mma chain of K = 80 yields
+// pieces of ||t||^2 against 1.0, and A is pre-scaled by -2, so that ONE wgmma chain of K = 80 yields
 //   acc(x,t) = ||t||^2 - 2 x.t      in fp32, to 2^-21 (||x||^2 + ||t||^2)   (all-pairs audit, tests/test_engine_gpu.py)
 // KNN only uses acc as a FILTER: a candidate is re-evaluated exactly (fp64, sklearn's summation order) iff
 // acc <= (worst kept distance - ||x||^2) + kappa (||x||^2 + ||t||^2), kappa = 2^-18; every row that could enter the k-slot heap
@@ -17,13 +17,12 @@
 // packed norm: B carries (1-kappa)||t||^2.)
 // KNN: spatial order and pruning.  The training rows are stored in kd order (create(): recursive median splits down to tiles
 // of 64), so a tile is a small ball (centre c_t, radius r_t).  A call first sorts its queries by HOME tile (the kd leaf a
-// query falls into: knn_key_kernel + a counting sort), so the 512 rows of a pass are neighbours too.  Per pass the producer
+// query falls into: knn_key_kernel + a counting sort), so the 256 rows of a pass are neighbours too.  Per pass the producer
 // walks the tiles by the distance of their centres from the pass's home tile and loads tile t only if
 //   (||x0 - c_t|| - r_t - rho)^2 <= H        x0 = first row of the pass, rho = max ||x - x0||, H = max current k-th distance^2
 // -- otherwise no row of t can be among the k nearest of any row of the pass (triangle inequality; all roundings taken in the
 // safe direction; H only falls, so a stale H is merely less sharp).  The epilogue repeats the test per lane with its own
-// ||x - x0|| and k-th distance and skips the TMEM read and the filter when no lane of the warp needs the tile.  On the bench
-// workload (10M queries x 50k rows, k = 5) a pass multiplies ~1/6 of the tiles.
+// ||x - x0|| and k-th distance and skips the accumulator read and the filter when no lane of the warp needs the tile.
 // Order independence.  The k smallest distances are the same SET whatever the visiting order, except when rows tie at the
 // k-th distance: there sklearn's answer depends on its heap's history.  The epilogue watches for rows left out at exactly the
 // final k-th distance; if such a row and the kept rows at that distance do not all carry one class, the query goes to the
@@ -47,8 +46,8 @@
 //       delta_d <= eps_mma M_j + 2^-20 xn + 2^-24 (xn + qn) + 2^-23 r_j sqrt(qn)
 //       M_j = r_j (2 sqrt(qn) + r_j + 2 |c'_j|) >= the sum of the absolute values of the MMA's products
 //     (qn = ||x'||^2, xn = ||x' - c'_j||^2, r_j = max ||u||; the 2^-24 / 2^-23 terms are the roundings of x' and u:
-//     the engine measures the distance from a point within 2^-24 |x - c0| of x), eps_mma = kSvcEpsMma is 4x the
-//     largest |acc - exact| / M_j the all-pairs audit observes (tests/test_engine_gpu.py), eta_const = 1.65e-6 covers
+//     the engine measures the distance from a point within 2^-24 |x - c0| of x), eps_mma = kSvcEpsMma is at least 2x the
+//     largest |acc - exact| / M_j the all-pairs audit observes (asserted by tests/test_engine_gpu.py), eta_const = 1.65e-6 covers
 //     ex2.approx (2^-22), the fp32 coefficient (2^-24), the fma that forms e where |e| <= 4 (ln2 2^-24 |e|) and the fp32
 //     sums: four chains of 16 terms per tile (15 u), their combination (2 u) and a compensated (Kahan) class sum (2 u);
 //   * E_p = 1.25 sum_j eta_j |tsum_j,m(p)| + Eabs_p,  Eabs_p = 1.04e-8 sum_s |coef_s| + 1e-9: where |e| > 4 the rounding of
@@ -58,37 +57,36 @@
 // change libsvm's first-maximum vote (svm.cpp:2893-2896); otherwise the kernel stores -1 - label and the fp64 kernel
 // re-evaluates exactly those rows in the same call (svc.cu, launch_svc_marked) -- the GaussianNB pattern of scorers.cu.
 //
-// Data layout.  create() packs the reference rows once into tile images of 64 rows x K=80 bf16 in the UMMA
+// Data layout.  create() packs the reference rows once into tile images of 64 rows x K=80 bf16 in the GMMA
 // canonical K-major / no-swizzle layout (8x8 core matrices of 128 B; LBO = 128 B along K, SBO = 1280 B along N),
 // followed (SVC) by the tile's dual coefficients [C-1][64] fp32, its centre c'_j and the two constants of eta_j.  A tile image is contiguous in HBM, so
-// one cp.async.bulk (TMA unit, UBLKCP) brings it into a shared-memory ring stage.  SVC classes start on tile
+// one cp.async.bulk (TMA unit) brings it into a shared-memory ring stage.  SVC classes start on tile
 // boundaries (padded with zero-coefficient rows).  KNN keeps a second fp64 copy of the training rows in tile order, padded to
-// 12 doubles (three 32-byte sectors, read with three 256-bit loads) for the exact re-evaluation; at 50k x 12 it is 4.8 MB and
+// 12 doubles (three 32-byte sectors, read with six 128-bit loads) for the exact re-evaluation; at 50k x 12 it is 4.8 MB and
 // stays in L2.  Pruning tables: tile centres and radii (fp64), the kd tree, and per home tile the list of all tiles by centre
 // distance (n_tiles^2 x 2 B, 1.2 MB at 782 tiles; models beyond 4096 tiles walk outwards from the home tile in kd order and
 // test every tile).
 //
-// Kernel (persistent).  SVC: 1 CTA / SM, 512 query rows per pass.  KNN: 2 CTAs / SM, 256 query rows per pass.
-//   KNN: warps 0-7, each thread owns ONE query row: packs it into the A operand (2 tiles of 128 x 80 bf16 in shared
-//               memory, same canonical layout), later reads its accumulator row from TMEM (tcgen05.ld 32x32b)
-//               and runs the filter epilogue on 64 columns per reference tile;
-//   SVC: warps 0-7, each thread owns TWO query rows (the same TMEM lane of two query tiles), so that one broadcast
-//               LDS.128 of dual coefficients feeds two rows: the coefficient loads were the kernel's bound (shared-memory
-//               return bandwidth, profiles/r01e), not the ex2 unit;
-//   next warp   streams reference tile images through a 4-stage (KNN: 3-stage) ring (bulk copy + mbarrier tx count); SVC: every
-//               tile in order, one lane; KNN: the whole warp computes which tiles the pass needs (see above), lane 0 loads them;
-//   last warp   runs warp-uniformly; one ELECTED lane issues 5 (K steps) tcgen05.mma M128 N64 K16 per query tile and reference
-//               tile into a double-buffered TMEM accumulator (query tiles x 2 buffers x 64 columns: SVC all 512 columns, KNN 256
-//               per CTA) and commits to the ring's "empty" barrier and the accumulator's "full" barrier.
-// Each reference tile (10 KB) is reused by all query rows of the pass.
+// Kernel (persistent, 1 CTA / SM, 256 query rows per pass = two query tiles of 128 rows in the A operand, same canonical
+// layout).  The epilogue warps form warpgroups; a warpgroup issues the wgmma itself (M64 N64 K16, 5 K steps per 64-row half
+// of a query tile, A and B from shared memory, fp32 accumulators in registers), waits for it, and every warp then transposes
+// its accumulator fragment through a private shared-memory buffer so that each thread sees whole accumulator rows:
+//   KNN: warps 0-7 (two warpgroups, one query tile each), each thread owns ONE query row: packs it into the A operand
+//               and runs the filter epilogue on the 64 columns of each reference tile;
+//   SVC: warps 0-3 (one warpgroup, both query tiles), each thread owns TWO query rows (one per query tile), so that one
+//               broadcast LDS.128 of dual coefficients feeds two rows;
+//   last warp   streams reference tile images through a 4-stage ring (bulk copy + mbarrier tx count); SVC: every tile in
+//               order, one lane; KNN: the whole warp computes which tiles the pass needs (see above), lane 0 loads them.
+// Thread t of warp w owns row 64 (t >> 4) + 16 (w & 3) + (t & 15) of its query tile: exactly the rows of the warp's share of
+// the two M64 accumulators, so the transpose stays inside the warp.  Each reference tile (10 KB) is reused by all query rows
+// of the pass.
 //
-// A hazard worth writing down (it cost a debugging session on the B200): an mbarrier.arrive does NOT wait for the
-// warp's outstanding ld.shared.  The SVC epilogue reads the dual coefficients out of the ring stage with plain
-// shared loads and then releases the stage; under MUFU pressure those loads can sit in the MIO queue for over a
-// microsecond, the arrive overtakes them, the producer's bulk copy refills the stage and the loads return the NEXT
-// tile's coefficients.  The release is therefore made data-dependent on the sums that consumed every coefficient
-// (a __threadfence_block() before the arrive works too and costs more).  tcgen05.ld needs no such care:
-// tcgen05.wait::ld is explicit.
+// A hazard worth writing down: an mbarrier.arrive does NOT wait for the warp's outstanding ld.shared.  The SVC epilogue
+// reads the dual coefficients out of the ring stage with plain shared loads and then releases the stage; under MUFU
+// pressure those loads can sit in the MIO queue for over a microsecond, the arrive overtakes them, the producer's bulk
+// copy refills the stage and the loads return the NEXT tile's coefficients.  The release is therefore made
+// data-dependent on the sums that consumed every coefficient (a __threadfence_block() before the arrive works too and
+// costs more).  The wgmma operands need no such care: wgmma.wait_group returns only once the MMAs have read them.
 #include <cuda_bf16.h>
 
 #include <algorithm>
@@ -104,27 +102,28 @@
 
 namespace tcsdn {
 
-constexpr int kEKnnWarps = 8;        // KNN epilogue warps (one query row per thread); two CTAs per SM
-constexpr int kESvcWarps = 8;        // SVC epilogue warps (two query rows per thread)
-constexpr int kEKnnThreads = (kEKnnWarps + 2) * 32;   // + producer warp + MMA warp
-constexpr int kESvcThreads = (kESvcWarps + 2) * 32;
-constexpr int kERows = 512;          // SVC: query rows per CTA pass (4 MMA tiles of 128)
-constexpr int kKnnRows = 256;        // KNN: query rows per CTA pass (2 MMA tiles of 128)
+constexpr int kEKnnWarps = 8;        // KNN epilogue warps (one query row per thread)
+constexpr int kESvcWarps = 4;        // SVC epilogue warps (two query rows per thread)
+constexpr int kEKnnThreads = (kEKnnWarps + 1) * 32;   // + producer warp
+constexpr int kESvcThreads = (kESvcWarps + 1) * 32;
+constexpr int kERows = 256;          // SVC: query rows per CTA pass (2 query tiles of 128)
+constexpr int kKnnRows = 256;        // KNN: query rows per CTA pass (2 query tiles of 128)
+constexpr int kETStride = 68;        // row stride (floats) of the per-warp accumulator transpose buffer: 16-byte aligned rows
+constexpr int kETBytes = 8 * 32 * kETStride * 4;   // transpose buffers: KNN 8 warps x 32 rows, SVC 4 warps x 64 rows
 constexpr int kEN = 64;              // reference rows per tile (MMA N)
 constexpr int kEK = 80;              // packed K
 constexpr int kEKSteps = kEK / 16;
 constexpr int kEMaxD = 12;           // 6 d + 6 <= 80
-constexpr int kEStages = 4;          // SVC ring depth (and the size of the barrier arrays)
-constexpr int kEKnnStages = 3;       // KNN ring depth: two CTAs share the SM's shared memory
+constexpr int kEStages = 4;          // ring depth
 constexpr int kETileB = kEN * kEK * 2;      // 10240 bytes of bf16 per reference tile
 constexpr int kEATile = 128 * kEK * 2;      // 20480 bytes per query tile
 constexpr int kESBO = (kEK / 8) * 128;      // 1280
 constexpr int kEMaxK = 32;                  // neighbours kept per query in the engine
-constexpr int kEMaxNC1 = 5;                 // SVC: n_classes - 1 (the per-pair sums and bounds of 512 rows live in shared memory)
-constexpr float kSvcEpsMma = 1.0f / 524288.0f;   // 2^-19: bound on |acc - exact| / M_j; 4x the all-pairs audit's maximum
+constexpr int kEMaxNC1 = 5;                 // SVC: n_classes - 1 (the per-pair sums and bounds of 256 rows live in shared memory)
+constexpr float kSvcEpsMma = 1.0f / 524288.0f;   // 2^-19: bound on |acc - exact| / M_j; >= 2x the all-pairs audit's maximum
 constexpr float kSvcEtaConst = 1.65e-6f;         // relative part of the K error that does not depend on distances (file header)
-constexpr float kKappa = 1.0f / 262144.0f;  // 2^-18: filter slack per unit of (||x||^2 + ||t||^2); 8x the largest error the
-                                            // all-pairs audit observes (2^-21.0 .. 2^-20.4, tests/test_engine_gpu.py)
+constexpr float kKappa = 1.0f / 262144.0f;  // 2^-18: filter slack per unit of (||x||^2 + ||t||^2); at least 4x the largest error
+                                            // the all-pairs audit observes (asserted by tests/test_engine_gpu.py)
 constexpr int kEListCap = 24;               // per-thread candidate list, 16-bit entries (tile offset, group of 8 columns, mask)
 constexpr int kEListRoom = 8;               // one tile appends at most this many: lists are evaluated beyond cap - room
 constexpr int kEMaxLeaves = 12000;           // KNN: kd leaves = bins of the query sort (a 48 KB shared-memory histogram)
@@ -243,81 +242,70 @@ __device__ __forceinline__ void e_bulk_g2s(void *dst, const void *src, uint32_t 
                  : "memory");
 }
 __device__ __forceinline__ uint64_t e_desc(uint32_t saddr) {
-    // K-major, SWIZZLE_NONE: start >> 4 | LBO(128 B) >> 4 << 16 | SBO(1280 B) >> 4 << 32 | version 1 << 46
-    return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)(128 >> 4) << 16) | ((uint64_t)(kESBO >> 4) << 32) | ((uint64_t)1 << 46);
+    // wgmma shared-memory descriptor, K-major, no swizzle: start >> 4 | LBO (128 B: next core matrix along K) >> 4 << 16 |
+    // SBO (1280 B: next 8 rows) >> 4 << 32; one K step of 16 advances the start by 256 B
+    return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)(128 >> 4) << 16) | ((uint64_t)(kESBO >> 4) << 32);
 }
-__device__ __forceinline__ void e_mma(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
+// the compiler must not move accesses of the accumulator registers across the wgmma fences / waits
+__device__ __forceinline__ void e_acc_fence(float (&d)[32]) {
+#pragma unroll
+    for (int i = 0; i < 32; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// d (+)= A[64 x 16] B[64 x 16]^T, both bf16 K-major in shared memory, fp32 accumulators (wgmma fragment layout)
+__device__ __forceinline__ void e_wgmma(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
     asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}\n" ::"r"(tmem_d),
-        "l"(da), "l"(db), "r"(idesc), "r"(accumulate)
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, "
+        "%14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(accumulate)
         : "memory");
 }
-// exactly one lane of a converged warp gets true (the pattern the compiler recognises for single-thread tcgen05 issue)
-__device__ __forceinline__ bool e_elect_one() {
-    uint32_t pred = 0;
-    asm volatile(
-        "{\n.reg .b32 rx;\n.reg .pred px;\n"
-        "elect.sync rx|px, 0xffffffff;\n"
-        "@px mov.s32 %0, 1;\n}\n"
-        : "+r"(pred));
-    return pred != 0;
-}
-__device__ __forceinline__ void e_commit(uint64_t *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(e_smem(bar)) : "memory");
-}
-__device__ __forceinline__ void e_tmem_ld32(uint32_t taddr, float (&v)[32]) {
-    uint32_t r[32];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// One query tile (128 rows at sAq) against one reference tile (64 rows at sBs), issued by the whole warpgroup: two M64
+// halves x 5 K steps, waited for.  Then each warp writes its share (rows 16 w .. 16 w + 15 of either half) to its transpose
+// buffer `tb` rows [0, 32) -- half h, fragment row i at row 16 h + i -- so that lane l finds its query row at row l.
+__device__ __forceinline__ void e_mma_tile(const unsigned char *sAq, const unsigned char *sBs, float *tb, int lane) {
+    float d0[32], d1[32];
 #pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
+    for (int i = 0; i < 32; ++i) { d0[i] = 0.f; d1[i] = 0.f; }
+    const uint32_t a0 = e_smem(sAq), b0 = e_smem(sBs);
+    e_acc_fence(d0);
+    e_acc_fence(d1);
+    asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+#pragma unroll
+    for (int k = 0; k < kEKSteps; ++k) e_wgmma(d0, e_desc(a0 + k * 256), e_desc(b0 + k * 256), k > 0);
+#pragma unroll
+    for (int k = 0; k < kEKSteps; ++k) e_wgmma(d1, e_desc(a0 + 8 * kESBO + k * 256), e_desc(b0 + k * 256), k > 0);
+    asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+    asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+    e_acc_fence(d0);
+    e_acc_fence(d1);
+    // fragment: d[4 g + {0,1}] = (row lane / 4, columns 8 g + 2 (lane % 4) + {0,1}), d[4 g + {2,3}] = the same 8 rows further
+    __syncwarp();   // the previous tile's rows have been read by every lane
+    float *r0 = tb + (lane >> 2) * kETStride + 2 * (lane & 3);
+#pragma unroll
+    for (int g = 0; g < 8; ++g) {
+        *reinterpret_cast<float2 *>(r0 + 8 * g) = make_float2(d0[4 * g], d0[4 * g + 1]);
+        *reinterpret_cast<float2 *>(r0 + 8 * kETStride + 8 * g) = make_float2(d0[4 * g + 2], d0[4 * g + 3]);
+        *reinterpret_cast<float2 *>(r0 + 16 * kETStride + 8 * g) = make_float2(d1[4 * g], d1[4 * g + 1]);
+        *reinterpret_cast<float2 *>(r0 + 24 * kETStride + 8 * g) = make_float2(d1[4 * g + 2], d1[4 * g + 3]);
+    }
+    __syncwarp();
 }
-// 32-column TMEM load without the wait (several loads in flight); e_tmem_wait_ld() + e_regs_fence32() order the uses
-__device__ __forceinline__ void e_tmem_ld32_issue(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
+// n consecutive accumulator values of one transposed row (16-byte loads)
+template <int N>
+__device__ __forceinline__ void e_ld_row(const float *p, uint32_t (&r)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; i += 4) {
+        const float4 v = *reinterpret_cast<const float4 *>(p + i);
+        r[i] = __float_as_uint(v.x); r[i + 1] = __float_as_uint(v.y); r[i + 2] = __float_as_uint(v.z); r[i + 3] = __float_as_uint(v.w);
+    }
 }
-__device__ __forceinline__ void e_tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// emits nothing: tells the compiler that r[] is (re)defined here, so no use of it can be scheduled before the wait above
-__device__ __forceinline__ void e_regs_fence32(uint32_t (&r)[32]) {
-    asm volatile(""
-                 : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]), "+r"(r[8]),
-                   "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15]), "+r"(r[16]),
-                   "+r"(r[17]), "+r"(r[18]), "+r"(r[19]), "+r"(r[20]), "+r"(r[21]), "+r"(r[22]), "+r"(r[23]), "+r"(r[24]),
-                   "+r"(r[25]), "+r"(r[26]), "+r"(r[27]), "+r"(r[28]), "+r"(r[29]), "+r"(r[30]), "+r"(r[31])
-                 :
-                 : "memory");
-}
-// 16-column TMEM load split into "issue" and "wait", so that the next chunk can be in flight while the current one is
-// processed.  The wait names the registers as in/out operands: the compiler must not touch them before it.
-__device__ __forceinline__ void e_tmem_ld16_issue(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void e_tmem_ld16_wait(uint32_t (&r)[16]) {
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-                 : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]), "+r"(r[8]),
-                   "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15])
-                 :
-                 : "memory");
-}
+// warpgroup-wide barrier (named barrier 1 + warpgroup)
+__device__ __forceinline__ void e_wg_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
 __device__ __forceinline__ int2 e_lds_v2(const void *p) {   // one 8-byte volatile shared load
     int2 r;
     asm volatile("ld.volatile.shared.v2.b32 {%0, %1}, [%2];" : "=r"(r.x), "=r"(r.y) : "r"(e_smem(p)) : "memory");
@@ -327,13 +315,16 @@ __device__ __forceinline__ void e_sts_v2(void *p, int2 v) {
     asm volatile("st.volatile.shared.v2.b32 [%0], {%1, %2};" ::"r"(e_smem(p)), "r"(v.x), "r"(v.y) : "memory");
 }
 
-// one padded fp64 row (12 doubles = 96 bytes, 32-byte aligned) through the read-only path: three 256-bit loads (LDG.E.256) --
-// a row is three 32-byte sectors, and with scattered rows it is sector requests that the L1 runs out of: 16-byte loads cost six
+// one padded fp64 row (12 doubles = 96 bytes, 32-byte aligned) through the read-only path: six 128-bit loads in one asm
+// block, so that the compiler keeps them together (one L2 round trip per row)
 __device__ __forceinline__ void e_ldg_row12(const double *p, double (&v)[12]) {
     asm volatile(
-        "ld.global.nc.v4.f64 {%0, %1, %2, %3}, [%12];\n\t"
-        "ld.global.nc.v4.f64 {%4, %5, %6, %7}, [%12+32];\n\t"
-        "ld.global.nc.v4.f64 {%8, %9, %10, %11}, [%12+64];"
+        "ld.global.nc.v2.f64 {%0, %1}, [%12];\n\t"
+        "ld.global.nc.v2.f64 {%2, %3}, [%12+16];\n\t"
+        "ld.global.nc.v2.f64 {%4, %5}, [%12+32];\n\t"
+        "ld.global.nc.v2.f64 {%6, %7}, [%12+48];\n\t"
+        "ld.global.nc.v2.f64 {%8, %9}, [%12+64];\n\t"
+        "ld.global.nc.v2.f64 {%10, %11}, [%12+80];"
         : "=d"(v[0]), "=d"(v[1]), "=d"(v[2]), "=d"(v[3]), "=d"(v[4]), "=d"(v[5]), "=d"(v[6]), "=d"(v[7]), "=d"(v[8]), "=d"(v[9]),
           "=d"(v[10]), "=d"(v[11])
         : "l"(p));
@@ -344,19 +335,12 @@ __device__ __forceinline__ float e_ex2(float x) {   // one MUFU.EX2 (2 ulp), flu
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
 }
-// packed fp32 FMA (FFMA2): acc.{x,y} += a.{x,y} * b.{x,y} in ONE issue slot
+// acc.{x,y} += a.{x,y} * b.{x,y}: two fp32 FMAs, each rounded once
 __device__ __forceinline__ void e_fma2(float2 &acc, const float2 a, const float2 b) {
-    unsigned long long d = *reinterpret_cast<unsigned long long *>(&acc);
-    const unsigned long long ua = *reinterpret_cast<const unsigned long long *>(&a);
-    const unsigned long long ub = *reinterpret_cast<const unsigned long long *>(&b);
-    asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(d) : "l"(ua), "l"(ub));
-    acc = *reinterpret_cast<float2 *>(&d);
+    acc.x = fmaf(a.x, b.x, acc.x);
+    acc.y = fmaf(a.y, b.y, acc.y);
 }
-__device__ __forceinline__ float e_min3(float a, float b, float c) {
-    float r;
-    asm("min.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c));   // FMNMX3
-    return r;
-}
+__device__ __forceinline__ float e_min3(float a, float b, float c) { return fminf(fminf(a, b), c); }
 
 // split an fp32 value into three bf16 pieces, exactly: x == h + m + l
 __host__ __device__ __forceinline__ void split3(float x, __nv_bfloat16 &h, __nv_bfloat16 &m, __nv_bfloat16 &l) {
@@ -405,7 +389,7 @@ __device__ __forceinline__ float knn_thr_base(double hv0, double qn) {
 }
 
 // ------------------------------------------------------------------------------------------------ KNN: query order
-// The queries of a call are grouped by HOME tile (the kd leaf they fall into) so that the 512 rows of a pass are neighbours:
+// The queries of a call are grouped by HOME tile (the kd leaf they fall into) so that the 256 rows of a pass are neighbours:
 // a counting sort in three kernels.  Block b owns the rows [b R, (b+1) R) in both passes over the rows.
 constexpr int kSortThreads = 512;
 
@@ -467,40 +451,8 @@ __global__ void __launch_bounds__(kSortThreads) knn_scatter_kernel(const int32_t
 }
 
 // ------------------------------------------------------------------------------------------------ the kernel
-// 8-column TMEM load (issue only) and the matching wait for two of them
-__device__ __forceinline__ void e_tmem_ld8_issue(uint32_t taddr, uint32_t (&r)[8]) {
-#if defined(TCSDN_EXP_NO_LDTM)   // experiment build: no TMEM loads (registers get the address instead)
-    for (int i = 0; i < 8; ++i) r[i] = 0xBF000000u + (taddr & 0xFFFFu) + i;
-    return;
-#endif
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-                 : "r"(taddr));
-}
-__device__ __forceinline__ void e_tmem_ld8_wait2(uint32_t (&r)[8], uint32_t (&q)[8]) {
-#if defined(TCSDN_EXP_NO_LDTM)
-    return;
-#endif
-    // no "memory" clobber: the register operands carry the dependency, and the compiler stays free to move coefficient
-    // loads and FMAs across the wait
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-                 : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]),
-                   "+r"(q[0]), "+r"(q[1]), "+r"(q[2]), "+r"(q[3]), "+r"(q[4]), "+r"(q[5]), "+r"(q[6]), "+r"(q[7]));
-}
-
-// two 16-column TMEM loads complete (both register sets are named as in/out operands: no use may move above the wait)
-__device__ __forceinline__ void e_tmem_ld16_wait2(uint32_t (&r)[16], uint32_t (&q)[16]) {
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-                 : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]), "+r"(r[8]),
-                   "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15]),
-                   "+r"(q[0]), "+r"(q[1]), "+r"(q[2]), "+r"(q[3]), "+r"(q[4]), "+r"(q[5]), "+r"(q[6]), "+r"(q[7]), "+r"(q[8]),
-                   "+r"(q[9]), "+r"(q[10]), "+r"(q[11]), "+r"(q[12]), "+r"(q[13]), "+r"(q[14]), "+r"(q[15]));
-    // no "memory" clobber: the register operands carry the dependency, and the compiler stays free to move the next
-    // chunk's coefficient loads and FMAs across the wait
-}
-
 // Load one query row, centre it on c0, round to fp32 (x'), split -2 x' into three bf16 pieces and write the row of the A
-// operand (query tile qt, TMEM lane rt).  Returns ||x'||^2 (fp64); xp receives x' (zeros for a dead row).
+// operand (query tile qt, row rt).  Returns ||x'||^2 (fp64); xp receives x' (zeros for a dead row).
 template <typename T, bool SVC>
 __device__ __forceinline__ double e_pack_row(const EngineArgs &A, const T *__restrict__ X, int64_t row, bool live,
                                              unsigned char *sA, int qt, int rt, float &nf, float (&xp)[kEMaxD]) {
@@ -546,11 +498,10 @@ __device__ __forceinline__ double e_pack_row(const EngineArgs &A, const T *__res
 #define KT_FLUSH(base, cond)
 #endif
 
-// KNN: what the producer, the MMA warp and the epilogue warps tell each other about the tiles of a pass
+// KNN: what the producer and the epilogue warps tell each other about the tiles of a pass
 constexpr int kEBarRegion = 3072;   // barriers (256 B) + KnnShared
 struct KnnShared {
-    int2 stageInfo[kEStages];        // producer -> MMA warp: (tile in the stage or -1 = end of pass, bits of its gap)
-    int2 accInfo[2];                 // MMA warp -> epilogue warps: the same for the accumulator buffer
+    int2 stageInfo[kEStages];        // producer -> epilogue warps: (tile in the stage or -1 = end of pass, bits of its gap)
     float warpH[kEKnnWarps];         // per epilogue warp: largest k-th distance^2 among its rows (rounded up), +inf at pass start
     unsigned rho_bits[2];            // by pass parity: largest distance of a row of the pass from the pass's first row (float bits)
     int chunkT[32];                  // producer scratch: the 32 tiles of a chunk and their gaps
@@ -562,52 +513,44 @@ static_assert(sizeof(KnnShared) + 256 <= kEBarRegion, "KnnShared does not fit");
 // AUDIT (SVC; KNN keeps its audit flag in NC1): a separate instantiation, because the audit indexes the accumulator registers
 // and x' dynamically, which would put them in local memory in the production kernel too
 template <typename T, bool SVC, int NC1, bool AUDIT = false>
-__global__ void __launch_bounds__(SVC ? kESvcThreads : kEKnnThreads, SVC ? 1 : 2)
+__global__ void __launch_bounds__(SVC ? kESvcThreads : kEKnnThreads, 1)
 engine_kernel(const __grid_constant__ EngineArgs A, const T *__restrict__ X, int32_t *__restrict__ labels,
               double *__restrict__ scores, unsigned long long *__restrict__ counters) {
-    constexpr int kEpi = SVC ? kESvcWarps : kEKnnWarps;   // epilogue warps; then the producer warp, then the MMA warp
+    constexpr int kEpi = SVC ? kESvcWarps : kEKnnWarps;   // epilogue warps (whole warpgroups); then the producer warp
     constexpr int kRows = SVC ? kERows : kKnnRows;        // query rows per pass
-    constexpr int kQT = kRows / 128;                      // query tiles (MMA M = 128)
-    constexpr int kSt = SVC ? kEStages : kEKnnStages;     // ring depth
-    constexpr uint32_t kTmemCols = kQT * 2 * kEN;         // double-buffered accumulators: SVC all 512 columns, KNN 256 (two CTAs per SM)
+    constexpr int kQT = kRows / 128;                      // query tiles of 128 rows
+    constexpr int kSt = kEStages;                         // ring depth
+    static_assert(kEpi % 4 == 0 && kEpi * 32 * (SVC ? 2 : 1) == kRows, "one query row per thread (SVC: two), whole warpgroups");
     extern __shared__ __align__(1024) unsigned char smem[];
     unsigned char *sA = smem;                                          // kQT x 20480
-    unsigned char *sB = smem + kQT * kEATile;                          // kSt x tile_bytes
+    float *sT = reinterpret_cast<float *>(smem + kQT * kEATile);       // kETBytes: per-warp accumulator transpose buffers
+    unsigned char *sB = smem + kQT * kEATile + kETBytes;               // kSt x tile_bytes
     uint64_t *bars = reinterpret_cast<uint64_t *>(sB + (size_t)kSt * A.tile_bytes);
-    uint64_t *fullB = bars, *emptyB = bars + kEStages, *accFull = bars + 2 * kEStages, *accEmpty = accFull + 2;
-    uint64_t *aFull = accEmpty + 2;
+    uint64_t *fullB = bars, *emptyB = bars + kEStages;
+    uint64_t *aFull = emptyB + kEStages;
     uint64_t *coefFree = aFull + 1;      // the epilogue warps are done with a stage's side data (SVC coefficients)
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(coefFree + kEStages);
-    // after the barriers -- KNN: [512 threads][kEListCap] candidate lists, then the heaps; SVC: [P][512] fp64 pair sums,
-    // then [P][512] fp32 error bounds
+    // after the barriers -- KNN: [256 threads][kEListCap] candidate lists, then the heaps; SVC: [P][256] fp64 pair sums,
+    // then [P][256] fp32 error bounds
     unsigned char *cand = reinterpret_cast<unsigned char *>(bars) + kEBarRegion;
     KnnShared *ks = reinterpret_cast<KnnShared *>(reinterpret_cast<unsigned char *>(bars) + 256);   // KNN only
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int64_t n_super = (A.n + kRows - 1) / kRows;
+    // epilogue threads: the row of its query tile(s) this thread owns (see the file header) and its warp's transpose buffer
+    const int rt = 64 * (lane >> 4) + 16 * (warp & 3) + (lane & 15);
+    float *tbuf = sT + (size_t)warp * (kRows / kEpi) * kETStride;
 
     if (tid == 0) {
         for (int s = 0; s < kEStages; ++s) {
             e_mbar_init(&fullB[s], 1);
-            e_mbar_init(&emptyB[s], 1);        // tcgen05.commit: the MMAs have read the stage
+            e_mbar_init(&emptyB[s], kEpi);     // every epilogue warp's wgmma has read the stage
             e_mbar_init(&coefFree[s], kEpi);   // every epilogue warp has read the stage's side data
-        }
-        for (int b = 0; b < 2; ++b) {
-            e_mbar_init(&accFull[b], 1);
-            e_mbar_init(&accEmpty[b], kEpi);
         }
         e_mbar_init(aFull, kEpi);
         if constexpr (!SVC) { ks->rho_bits[0] = 0u; ks->rho_bits[1] = 0u; }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == kEpi + 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(e_smem(tmem_slot)), "r"(kTmemCols));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
 
     if (warp == kEpi) {
         // ------------------------------------------------------------------ reference tile producer
@@ -741,79 +684,16 @@ engine_kernel(const __grid_constant__ EngineArgs A, const T *__restrict__ X, int
             if (lane == 0 && counters) { atomicAdd(counters + 2, n_mult); atomicAdd(counters + 3, (unsigned long long)pass); }
             KT_FLUSH(0, lane == 0 && counters);
         }
-    } else if (warp == kEpi + 1) {
-        // ------------------------------------------------------------------ MMA issuer
-        // The whole warp runs this loop (warp-uniform control flow, so descriptors live in uniform registers) and ONE
-        // elected lane issues.  Issuing from `if (lane == 0)` instead makes the compiler wrap every tcgen05.mma in an
-        // ELECT / BRA.U.ANY serialisation loop: 215 instructions per reference tile for 20 MMAs, on an issue port shared
-        // with four epilogue warps -- that, not the tensor pipe, was the engine's critical path (ncu, profiles/r01c).
-        // instruction descriptor: D = F32, A = B = BF16, both K-major, N >> 3 at bit 17, M >> 4 at bit 24
-        const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(kEN >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-        // shared-memory descriptor: K-major, SWIZZLE_NONE; high word = SBO(1280 B) >> 4 | version 1 << 14, low word =
-        // start >> 4 | LBO(128 B) >> 4 << 16; one K step of 16 advances the start by 256 B = 16 units
-        const uint64_t desc_hi = ((uint64_t)(kESBO >> 4) | ((uint64_t)1 << 14)) << 32;
-        const uint32_t a_lo = ((e_smem(sA) >> 4) & 0x3FFFu) | ((128u >> 4) << 16);
-        uint32_t g = 0, pass = 0;
-        KT_DECL;
-        for (int64_t st = blockIdx.x; st < n_super; st += gridDim.x, ++pass) {
-            KT_START();
-            e_mbar_wait(aFull, pass & 1);   // the 512 query rows of this pass are packed
-            KT_STOP(0);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            // SVC: every tile, in order.  KNN: whatever the producer sends, until the stage that carries -1
-            for (int j = 0; SVC ? j < A.n_tiles : true; ++j, ++g) {
-                const uint32_t s = g % kSt, ph = (g / kSt) & 1;
-                const uint32_t b = g & 1, bph = (g >> 1) & 1;
-                KT_START();
-                if constexpr (SVC) e_mbar_wait(&fullB[s], ph); else e_mbar_poll(&fullB[s], ph);
-                KT_STOP(1);
-                int2 info = make_int2(0, 0);
-                if constexpr (!SVC) info = e_lds_v2(&ks->stageInfo[s]);
-                const bool last = !SVC && info.x < 0;
-                KT_START();
-                if constexpr (SVC) e_mbar_wait(&accEmpty[b], bph ^ 1); else e_mbar_poll(&accEmpty[b], bph ^ 1);
-                KT_STOP(2);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                if (e_elect_one()) {
-                    if constexpr (!SVC) e_sts_v2(&ks->accInfo[b], info);
-                    if (!last) {
-                        const uint32_t b_lo = ((e_smem(sB + (size_t)s * A.tile_bytes) >> 4) & 0x3FFFu) | ((128u >> 4) << 16);
-#pragma unroll
-                        for (int t = 0; t < kQT; ++t) {
-                            const uint32_t dcol = tmem_base + (uint32_t)((t * 2 + b) * kEN);
-#pragma unroll
-#if defined(TCSDN_EXP_NO_MMA)     // experiment build: no MMA at all (commits only)
-                            for (int k = 0; k < 0; ++k)
-#elif defined(TCSDN_EXP_ONE_MMA)  // experiment build: one K step instead of five (a fifth of the operand reads)
-                            for (int k = 0; k < 1; ++k)
-#else
-                            for (int k = 0; k < kEKSteps; ++k)
-#endif
-                                e_mma(dcol, desc_hi | (uint64_t)(a_lo + (uint32_t)(t * (kEATile >> 4) + k * 16)),
-                                      desc_hi | (uint64_t)(b_lo + (uint32_t)(k * 16)), idesc, k > 0);
-                        }
-                        e_commit(&emptyB[s]);    // smem stage may be refilled once these MMAs have read it
-                    } else {
-                        e_mbar_arrive(&emptyB[s]);   // nothing reads the end-of-pass stage
-                    }
-                    e_commit(&accFull[b]);   // accumulators of this reference tile are complete (end of pass: nothing pending)
-                }
-                __syncwarp();
-                if (last) { ++g; break; }
-            }
-        }
-        KT_FLUSH(8, !SVC && lane == 0 && counters);
     } else if constexpr (!SVC) {
-        // ------------------------------------------------------------------ KNN: 512 query-row owners (pack A, filter epilogue)
-        const int qt = warp >> 2;                           // query tile 0..3
-        const int rt = (warp & 3) * 32 + lane;              // row inside the tile == TMEM lane
-        const uint32_t lane_addr = (uint32_t)((warp & 3) * 32) << 16;
+        // ------------------------------------------------------------------ KNN: 256 query-row owners (pack A, wgmma, filter epilogue)
+        const int qt = warp >> 2;                           // query tile 0..1 = this thread's warpgroup
         const bool prune = A.qperm != nullptr;
         uint32_t g = 0, pass = 0;
         float nf = 0.f;
         KT_DECL;
         for (int64_t st = blockIdx.x; st < n_super; st += gridDim.x, ++pass) {
             KT_START();
+            e_wg_sync(qt);                                  // the warpgroup's last wgmma of the previous pass has read sA
             const int64_t slot = st * kRows + qt * 128 + rt;
             const bool live = slot < A.n;
             const int64_t row = !live ? 0 : (A.qperm ? (int64_t)A.qperm[slot] : slot);   // the query this thread owns
@@ -839,9 +719,10 @@ engine_kernel(const __grid_constant__ EngineArgs A, const T *__restrict__ X, int
                 }
                 if (tid == 0) ks->rho_bits[(pass + 1) & 1] = 0u;   // the other parity's slot is idle during this pass
             }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to UMMA
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to wgmma
             __syncwarp();
             if (lane == 0) e_mbar_arrive(aFull);
+            e_wg_sync(qt);                                  // the query tile is complete
             KT_STOP(0);
 
             {
@@ -878,7 +759,6 @@ engine_kernel(const __grid_constant__ EngineArgs A, const T *__restrict__ X, int
                 int32_t *myseq = ks->seqTile[warp];
                 int cnt = 0, base_seq = 0, next_round = 1, j = 0;
                 bool end = false;
-                const uint32_t taddr0 = tmem_base + lane_addr + (uint32_t)(qt * 2 * kEN);
                 auto tie_note = [&](double v, int32_t pos) {   // a row left out of the heap at the root's value v
                     const int c = A.ypos[pos];
                     if (v != tie_val) { tie_val = v; tie_cls = c; }
@@ -957,28 +837,28 @@ engine_kernel(const __grid_constant__ EngineArgs A, const T *__restrict__ X, int
                     }
                     if (end) break;
                     // ---- the next tile of the pass (or its end)
-                    const uint32_t b = g & 1, bph = (g >> 1) & 1;
+                    const uint32_t s = g % kSt, ph = (g / kSt) & 1;
                     ++g;
                     KT_START();
-                    e_mbar_poll(&accFull[b], bph);
+                    e_mbar_poll(&fullB[s], ph);
                     KT_STOP(2);
                     KT_START();
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    const int2 info = e_lds_v2(&ks->accInfo[b]);
+                    const int2 info = e_lds_v2(&ks->stageInfo[s]);
                     if (info.x < 0) {                       // end of pass (the branch on info also orders the load before the arrive)
-                        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
                         __syncwarp();
-                        if (lane == 0) e_mbar_arrive(&accEmpty[b]);
+                        if (lane == 0) e_mbar_arrive(&emptyB[s]);
                         end = true;
                         continue;
                     }
+                    // the whole warpgroup multiplies its query tile by the reference tile (wgmma is warpgroup-collective, so no
+                    // warp may skip it); once it has completed the stage goes back to the producer
+                    e_mma_tile(sA + qt * kEATile, sB + (size_t)s * A.tile_bytes, tbuf, lane);
+                    if (lane == 0) e_mbar_arrive(&emptyB[s]);
                     // this row cannot gain a neighbour from the tile: ||x - t|| >= ||x0 - t|| - ||x - x0|| >= gap - e > sqrt(k-th distance^2)
                     const float mgn = __fsub_rd(__int_as_float(info.y), e_up);
                     const bool far = !live || (!kAudit && prune && mgn > 0.f && __fmul_rd(mgn, mgn) > hv0f);
                     if (lane == 0) myseq[j - base_seq] = info.x;
-                    if (__all_sync(0xffffffffu, far)) {     // nobody in the warp needs the tile: release the buffer unread
-                        __syncwarp();
-                        if (lane == 0) e_mbar_arrive(&accEmpty[b]);
+                    if (__all_sync(0xffffffffu, far)) {     // nobody in the warp needs the tile: leave the accumulators unread
                         ++j;
                         KT_STOP(3);
                         continue;
@@ -987,17 +867,10 @@ engine_kernel(const __grid_constant__ EngineArgs A, const T *__restrict__ X, int
                     float thr = far ? -FLT_MAX : (kAudit ? FLT_MAX : thr_base);
                     const uint32_t etile = (uint32_t)(j - base_seq) << 11;
                     uint32_t lp = e_smem(mylist) + 2u * (uint32_t)cnt;   // 32-bit shared address of the list's tail
-                    // all 64 accumulator values go to registers at once and the TMEM buffer is released right away: what a
-                    // warp then does with them (group visits, an evaluation round) no longer holds up the next tile's MMAs
+                    // this thread's accumulator row, all 64 values
                     uint32_t r0[32], r1[32];
-                    e_tmem_ld32_issue(taddr0 + b * kEN, r0);
-                    e_tmem_ld32_issue(taddr0 + b * kEN + 32, r1);
-                    e_tmem_wait_ld();
-                    e_regs_fence32(r0);
-                    e_regs_fence32(r1);
-                    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                    __syncwarp();
-                    if (lane == 0) e_mbar_arrive(&accEmpty[b]);   // TMEM buffer may be overwritten
+                    e_ld_row(tbuf + lane * kETStride, r0);
+                    e_ld_row(tbuf + lane * kETStride + 32, r1);
                     if constexpr (kHeapSmem && !kAudit) {
                         // No threshold yet (the pass's first tile): instead of re-evaluating all 64 rows exactly, take the k-th
                         // smallest ACCUMULATOR value s: the k-th smallest exact distance of the tile is at most
@@ -1107,22 +980,20 @@ engine_kernel(const __grid_constant__ EngineArgs A, const T *__restrict__ X, int
         KT_FLUSH(16, lane == 0 && counters);
         if (A.flag && nf != nf) atomicOr(A.flag, 1);
     } else {
-        // ------------------------------------------------------------------ SVC: 8 warps x 2 query rows per thread
+        // ------------------------------------------------------------------ SVC: 4 warps x 2 query rows per thread
         // Every support-vector tile carries its own centre c'_j (tiles are spatially compact, see create()):
         //   acc = ||u||^2 - 2 (x' - c'_j).u,  u = (s - c0) - c'_j   (B holds u and the scalar 2 c'_j.u per row)
         //   d   = ||x' - c'_j||^2 + acc ,  ||x' - c'_j||^2 summed directly in fp32 (no cancellation)
-        // A warp covers one TMEM lane quadrant of TWO query tiles, so one broadcast LDS.128 of coefficients serves both rows.
+        // A thread owns row rt of BOTH query tiles, so one broadcast LDS.128 of coefficients serves both rows.
         constexpr int C = NC1 + 1, P = C * NC1 / 2;
-        const int quad = warp & 3, hsel = warp >> 2;
-        const int rt = quad * 32 + lane;
-        const uint32_t lane_addr = (uint32_t)(quad * 32) << 16;
-        double *decS = reinterpret_cast<double *>(cand);            // [P][512]: sum over finished classes of coef K
-        float *errS = reinterpret_cast<float *>(decS + P * kERows); // [P][512]: the matching error bound
-        const int slot0 = (2 * hsel) * 128 + rt;                    // this thread's rows sit at slot0 and slot0 + 128
+        double *decS = reinterpret_cast<double *>(cand);            // [P][256]: sum over finished classes of coef K
+        float *errS = reinterpret_cast<float *>(decS + P * kERows); // [P][256]: the matching error bound
+        const int slot0 = rt;                                       // this thread's rows sit at slot0 and slot0 + 128
         const float g2 = A.g2;
         uint32_t g = 0;
         float nf = 0.f;
         for (int64_t st = blockIdx.x; st < n_super; st += gridDim.x) {
+            e_wg_sync(0);                                   // the last wgmma of the previous pass has read sA
             int64_t row[2];
             bool live[2];
             float xp[2][kEMaxD], sq[2], c2row[2];
@@ -1130,16 +1001,17 @@ engine_kernel(const __grid_constant__ EngineArgs A, const T *__restrict__ X, int
             for (int r = 0; r < 2; ++r) {
                 row[r] = st * kERows + slot0 + r * 128;
                 live[r] = row[r] < A.n;
-                const double qn = e_pack_row<T, true>(A, X, row[r], live[r], sA, 2 * hsel + r, rt, nf, xp[r]);
+                const double qn = e_pack_row<T, true>(A, X, row[r], live[r], sA, r, rt, nf, xp[r]);
                 const float qnf = __double2float_ru(qn);
                 sq[r] = __fsqrt_ru(qnf);
                 c2row[r] = A.svc_c2 * qnf;
 #pragma unroll
                 for (int p = 0; p < P; ++p) { decS[p * kERows + slot0 + r * 128] = 0.0; errS[p * kERows + slot0 + r * 128] = 0.f; }
             }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to UMMA
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to wgmma
             __syncwarp();
             if (lane == 0) e_mbar_arrive(aFull);
+            e_wg_sync(0);                                   // both query tiles are complete
 
             // Per (row, coefficient row): FOUR fp32 partial sums per tile (even / odd columns x even / odd groups of four
             // columns: chains of 16 terms, two FFMA2 accumulators), combined once per tile and added to the class sum with a
@@ -1169,20 +1041,20 @@ engine_kernel(const __grid_constant__ EngineArgs A, const T *__restrict__ X, int
 #pragma unroll 1
             for (int j = 0; j < A.n_tiles; ++j, ++g) {
                 const uint32_t sidx = g % kEStages;
-                const uint32_t b = g & 1, bph = (g >> 1) & 1;
                 const int cls = A.tile_class[j];
                 if (cls != cur_class) { flush_class(cur_class); cur_class = cls; }   // uniform: support vectors are grouped by class
-                e_mbar_wait(&accFull[b], bph);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t taddr0 = tmem_base + lane_addr + (uint32_t)(((2 * hsel) * 2 + b) * kEN);
-                const uint32_t taddr1 = taddr0 + 2 * kEN;          // the second row's query tile
-                // accumulator columns arrive in chunks of 8 per row, double-buffered (32 registers)
-                uint32_t va0[8], va1[8], vb0[8], vb1[8];
-                e_tmem_ld8_issue(taddr0, va0);
-                e_tmem_ld8_issue(taddr1, va1);
-                // the coefficients and the tile header were written by the bulk copy (async proxy): observe ITS barrier
-                // before reading them (already complete here -- the MMAs consumed the same stage -- so this never blocks)
+                // the tile image (B operand, coefficients, header) was written by the bulk copy: observe its barrier
                 e_mbar_wait(&fullB[sidx], (g / kEStages) & 1);
+                // both query tiles against the tile (warpgroup-collective); rows of query tile r land in rows [32 r, 32 r + 32)
+                // of the warp's transpose buffer
+                e_mma_tile(sA, sB + (size_t)sidx * A.tile_bytes, tbuf, lane);
+                e_mma_tile(sA + kEATile, sB + (size_t)sidx * A.tile_bytes, tbuf + 32 * kETStride, lane);
+                if (lane == 0) e_mbar_arrive(&emptyB[sidx]);
+                const float *trow0 = tbuf + lane * kETStride, *trow1 = trow0 + 32 * kETStride;
+                // accumulator columns are taken in chunks of 8 per row, double-buffered (32 registers)
+                uint32_t va0[8], va1[8], vb0[8], vb1[8];
+                e_ld_row(trow0, va0);
+                e_ld_row(trow1, va1);
                 const float *coef = reinterpret_cast<const float *>(sB + (size_t)sidx * A.tile_bytes + kETileB);
                 const float4 *hdr = reinterpret_cast<const float4 *>(coef + NC1 * kEN);   // c'_j [12], eta constants
                 float xn[2] = {0.f, 0.f};   // ||x' - c'_j||^2 summed directly in fp32
@@ -1225,7 +1097,7 @@ engine_kernel(const __grid_constant__ EngineArgs A, const T *__restrict__ X, int
                 // lists the NA active rows; the body below is instantiated for NA = 1 .. NC1.
                 // One block = 4 support-vector columns x 2 rows: NA broadcast LDS.128 of coefficients, 4 FFMA2 for the
                 // exponents, 8 MUFU.EX2, 4 NA FFMA2 into the chains.  The coefficients of block b + 1 are loaded before block b is
-                // computed (explicit double buffer: shared-memory latency was what the FFMA2s waited for, profiles/r02).
+                // computed (explicit double buffer: otherwise the FMAs wait for shared-memory latency).
                 auto load_cf = [&](float4 (&cf)[NA], int col) {
 #pragma unroll
                     for (int m = 0; m < NA; ++m)
@@ -1245,7 +1117,7 @@ engine_kernel(const __grid_constant__ EngineArgs A, const T *__restrict__ X, int
                         float2 e01 = bias2[r], e23 = bias2[r];
                         e_fma2(e01, make_float2(__uint_as_float(v[0]), __uint_as_float(v[1])), g22);
                         e_fma2(e23, make_float2(__uint_as_float(v[2]), __uint_as_float(v[3])), g22);
-#if defined(TCSDN_EXP_NO_EX2)   // experiment build: no MUFU (tools/gpu_svc_variants.sh)
+#if defined(TCSDN_EXP_NO_EX2)   // experiment build (-DTCSDN_EXP_NO_EX2, never the product): no MUFU
                         k.k01[r] = e01; k.k23[r] = e23;
 #else
                         k.k01[r] = make_float2(e_ex2(e01.x), e_ex2(e01.y));
@@ -1273,9 +1145,8 @@ engine_kernel(const __grid_constant__ EngineArgs A, const T *__restrict__ X, int
                 // stalled warp leaves the MUFU unit idle).
                 float4 cfA[NA], cfB[NA];
                 load_cf(cfA, 0);
-                e_tmem_ld8_wait2(va0, va1);
-                e_tmem_ld8_issue(taddr0 + 8, vb0);
-                e_tmem_ld8_issue(taddr1 + 8, vb1);
+                e_ld_row(trow0 + 8, vb0);
+                e_ld_row(trow1 + 8, vb1);
                 K4 kA = exps(va0, va1), kB;
 #pragma unroll
                 for (int cc = 0; cc < 8; ++cc) {           // chunk cc = columns 8 cc .. 8 cc + 7
@@ -1315,19 +1186,13 @@ engine_kernel(const __grid_constant__ EngineArgs A, const T *__restrict__ X, int
                     kB = exps(c0 + 4, c1 + 4);              // second half of this chunk
                     sums(cfA, kA, false);
                     if (cc < 7) {
-                        e_tmem_ld8_wait2(n0, n1);           // next chunk has landed
-                        if (cc == 6) {                      // ... and it was the last one: the TMEM buffer may be overwritten
-                            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                            __syncwarp();
-                            if (lane == 0) e_mbar_arrive(&accEmpty[b]);
-                        }
                         load_cf(cfA, 8 * cc + 8);
                         kA = exps(n0, n1);
                     }
                     sums(cfB, kB, true);
                     if (cc < 6) {                           // this chunk's registers are free: fetch the chunk after the next
-                        e_tmem_ld8_issue(taddr0 + 8 * (cc + 2), c0);
-                        e_tmem_ld8_issue(taddr1 + 8 * (cc + 2), c1);
+                        e_ld_row(trow0 + 8 * (cc + 2), c0);
+                        e_ld_row(trow1 + 8 * (cc + 2), c1);
                     }
                 }
                 // tile sums: combine the four chains of every active row, then Kahan-add to the class sum of the coefficient row it
@@ -1411,9 +1276,6 @@ engine_kernel(const __grid_constant__ EngineArgs A, const T *__restrict__ X, int
         }
         if (A.flag && nf != nf) atomicOr(A.flag, 1);
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == kEpi + 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kTmemCols));
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -1766,7 +1628,7 @@ bool engine_usable(const tcsdn_model *m, int64_t n, bool want_scores) {
         if (want_scores != (m->opt_engine >= 3)) return false; // decision values: fp64 kernel; audit modes fill scores
     } else if (m->opt_engine == 4) return false;
     if (m->opt_engine >= 2) return true;
-    return n >= 4096;   // below this the fp64 CUDA-core kernels (latency path) are faster than filling 148 SMs x 512 rows
+    return n >= 4096;   // below this the fp64 CUDA-core kernels (latency path) are faster than filling every SM with 256-row passes
 }
 
 template <typename T>
@@ -1792,7 +1654,7 @@ static int launch_engine_t(tcsdn_model *m, const T *x, int64_t n, int32_t *label
     for (int p = 0; p < (kEMaxNC1 + 1) * kEMaxNC1 / 2; ++p) A.svc_eabs[p] = E->eabs[p];
     const bool heap_smem = !svc && m->k <= kEHeapSmemK;
     const int P = m->n_classes * (m->n_classes - 1) / 2;
-    // KNN: order the queries by home tile (counting sort on this stream) so that a pass's 512 rows are neighbours and the
+    // KNN: order the queries by home tile (counting sort on this stream) so that a pass's 256 rows are neighbours and the
     // producer can leave out the tiles that are too far for all of them.  Scratch comes from the engine's own stream-ordered
     // pool (capturable into a CUDA graph, private to the call).
     A.ypos = E->d_ypos; A.tcent = E->d_tcent; A.trad = E->d_trad; A.chunk_lb = E->d_chunk_lb; A.tile_tn = E->d_tile_tn;
@@ -1834,11 +1696,11 @@ static int launch_engine_t(tcsdn_model *m, const T *x, int64_t n, int32_t *label
         }
     }
     const int rows_per_pass = svc ? kERows : kKnnRows;
-    const size_t smem = (size_t)(rows_per_pass / 128) * kEATile + (size_t)(svc ? kEStages : kEKnnStages) * E->tile_bytes + kEBarRegion +
+    const size_t smem = (size_t)(rows_per_pass / 128) * kEATile + kETBytes + (size_t)kEStages * E->tile_bytes + kEBarRegion +
                         (svc ? (size_t)P * kERows * (sizeof(double) + sizeof(float))
                              : kKnnRows * (size_t)kEListCap * sizeof(uint16_t) + (heap_smem ? kKnnRows * (size_t)m->k * 12 : 0));
     const int64_t n_super = (n + rows_per_pass - 1) / rows_per_pass;
-    const unsigned grid = (unsigned)std::min<int64_t>(n_super, (int64_t)m->sm_count * (svc ? 1 : 2));
+    const unsigned grid = (unsigned)std::min<int64_t>(n_super, (int64_t)m->sm_count);
 #define TCSDN_LAUNCH(SVCF, NC)                                                                                    \
     {                                                                                                             \
         auto kern = (SVCF && A.maxratio) ? engine_kernel<T, SVCF, NC, SVCF> : engine_kernel<T, SVCF, NC, false>;   \
@@ -1902,8 +1764,8 @@ void engine_read_stats(const tcsdn_model *m, int64_t *out) {
 #if defined(TCSDN_EXP_KNN_TIMING)
     unsigned long long kt[32];
     if (cudaMemcpy(kt, E->d_counters, sizeof(kt), cudaMemcpyDeviceToHost) == cudaSuccess) {
-        static const char *names[3] = {"producer (lane 0): aFull wait, pass setup, chunk gaps, emptyB wait", "mma warp: aFull wait, fullB wait, accEmpty wait",
-                                       "epilogue (16 lane-0s): pack, rounds, accFull wait, skipped tiles, filtered tiles, votes"};
+        static const char *names[3] = {"producer (lane 0): aFull wait, pass setup, chunk gaps, emptyB wait", "(unused)",
+                                       "epilogue (8 lane-0s): pack, rounds, fullB wait, skipped tiles, filtered tiles, votes"};
         for (int r = 0; r < 3; ++r) {
             fprintf(stderr, "KT %s:", names[r]);
             for (int i = 0; i < 8; ++i) fprintf(stderr, " %.3e", (double)kt[8 + r * 8 + i]);

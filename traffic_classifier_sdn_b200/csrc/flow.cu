@@ -47,7 +47,7 @@ int launch_flow_update(double *state, const double *packets, const double *bytes
                        const uint8_t *dir, int64_t n, void *features_out, int feat_dtype, cudaStream_t st) {
     if (n == 0) return TCSDN_OK;
     int64_t blocks = (n + 255) / 256;
-    if (blocks > 148 * 8) blocks = 148 * 8;
+    if (blocks > 132 * 8) blocks = 132 * 8;
     if (feat_dtype == TCSDN_F32)
         flow_update_kernel<float><<<(unsigned)blocks, 256, 0, st>>>(state, packets, bytes, curr_time, dir, n,
                                                                     static_cast<float *>(features_out));

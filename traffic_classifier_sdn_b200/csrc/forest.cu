@@ -502,9 +502,8 @@ static int launch_forest_cfg(tcsdn_model *m, const T *x, int64_t n, int32_t *lab
 template <typename T>
 static int launch_forest_t(tcsdn_model *m, const T *x, int64_t n, int32_t *labels, double *scores, int32_t *flag,
                            cudaStream_t st) {
-    // threads x rows-per-thread.  Measured on the 100-tree sklearn forest (12.5M rows): 256 x 4 -> 3.8e8 rows/s,
-    // 512 x 2 -> 6.3e8, 1024 x 1 -> 8.2e8: the walk is a chain of dependent shared-memory loads, and 32 warps hide its
-    // latency better than instruction-level parallelism inside 8 or 16.  TCSDN_OPT_FOREST_SHAPE (1, 2) selects the others.
+    // threads x rows-per-thread.  The walk is a chain of dependent shared-memory loads, so the default is the most warps
+    // (1024 x 1): warps hide its latency, where more rows per thread would only add instruction-level parallelism.  TCSDN_OPT_FOREST_SHAPE (1, 2) selects the others.
     // Forests whose trees do not fit the shared-memory buffer are walked in L2 / HBM: there the chain of dependent GLOBAL
     // gathers wants as many chains in flight per SM as possible -- 512 x 2 with two CTAs per SM (2 048 chains) --
     // TCSDN_OPT_FOREST_SHAPE = 3 forces 1024 x 1 for them too.

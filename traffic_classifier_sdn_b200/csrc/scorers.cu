@@ -17,8 +17,8 @@
 // GaussianNB costs two DFMA per (class, feature) instead of sub, mul, div, add:
 //   t = x * s - theta * s,  s = 1/sqrt(2 var)   (one rounding; theta*s is rounded once on the host)
 //   jll -= t * t
-// The B200 issues 64 DFMA/clk/SM, which makes a 6-class, 8-feature row cost 1.5 clk of fp64 pipe against
-// 1.1 clk of HBM time: the three-operation form was fp64-pipe-bound (ncu r01a: fp64 pipe 62 %, DRAM 22 %).
+// At 64 DFMA/clk/SM the three-operation form costs a 6-class, 8-feature row more fp64-pipe time than the two-DFMA form,
+// which keeps the fp64 pipe off the critical path of an HBM stream.
 // Error: |delta t| <= u |theta s| + u |t|, i.e. the joint log likelihood is exact to ~1e-16 * (theta/sigma)
 // relative to its own terms (<= 1e-11 of the row's largest |jll| in the tests, labels unchanged).
 #include <cfloat>
@@ -126,8 +126,8 @@ __device__ __forceinline__ void score_rows(const ScorerParams &P, const double (
 }
 
 // GaussianNB labels from an fp32 pre-pass with a rigorous error bound; rows it cannot certify are re-run in fp64 by
-// the caller, so the labels are those of the fp64 definition, always.  (The kernel was fp64-pipe-bound: 96 DFMA per
-// row at 64/clk/SM is 5.3 us per 1M rows, as long as the HBM transfer it should hide behind.)
+// the caller, so the labels are those of the fp64 definition, always.  (In fp64 the 96 DFMA per row take the fp64
+// pipe about as long as the HBM transfer they should hide behind.)
 //   fp64 definition   t = x a - b,  jll_c = c_c - sum_j t^2        (one rounding per fma, 2^-53: negligible here)
 //   fp32 pre-pass     the same with a, b, c rounded to fp32 and fp32 fma: t~, acc~
 //   |t~ - t| <= 2^-24 (|x a| + |b| + |t~|) <= 2^-23 (|t~| + |b|)          since |x a| + |b| <= |t| + 2 |b|
@@ -135,12 +135,9 @@ __device__ __forceinline__ void score_rows(const ScorerParams &P, const double (
 //   => |acc~_c - jll_c| <= E_c = 2^-19 (T_c + |c_c| + sum_j b_cj^2)       (1.45x slack), with T_c = c~_c - acc~_c for free
 // A row is certified when  acc~_best - E_best > acc~_c + E_c  for every other class: then jll_best > jll_c strictly, the
 // fp64 argmax is `best` and no tie rule is involved.  NaN/inf anywhere fails the comparison and lands in the fp64 path.
-// packed fp32 FMA (FFMA2): d.{x,y} = a.{x,y} * b.{x,y} + c.{x,y} in ONE issue slot
+// d.{x,y} = a.{x,y} * b.{x,y} + c.{x,y}: two fp32 FMAs, each rounded once
 __device__ __forceinline__ float2 fma2(const float2 a, const float2 b, const float2 c) {
-    unsigned long long d;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(*reinterpret_cast<const unsigned long long *>(&a)),
-        "l"(*reinterpret_cast<const unsigned long long *>(&b)), "l"(*reinterpret_cast<const unsigned long long *>(&c)));
-    return *reinterpret_cast<float2 *>(&d);
+    return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
 }
 
 template <int D, int R, int kRPT>
@@ -149,9 +146,7 @@ __device__ __forceinline__ void gnb_prepass_rows(const ScorerParams &P, const fl
     // hi/lo = acc -/+ E with E = eps (c + k - acc):  hi = acc (1 - eps) + eps (c + k),  lo = acc (1 + eps) - eps (c + k): one
     // fma each (their own rounding, 2^-24 |acc|, is 1/32 of E: inside the slack).  The class with the largest hi is the
     // only one that can be certified, and it is iff its lo beats every other hi.
-    // Two rows per instruction: an FFMA2 does the t = x a - b and T += t^2 of two rows in one issue slot (ncu r02 showed issue
-    // 68 %, FMA pipe 36 % on this kernel; halving the FMA issue slots changed neither the 1M-row step nor the 100M-row batch --
-    // 51.4 / 77.0 % against 51.8 / 77.3 % -- so issue is not the limiter either; kept because it is no more code).
+    // Rows are scored in pairs (fma2: the t = x a - b and T += t^2 of two rows side by side).
     // T = sum t^2 is accumulated first and acc = c - T formed once: at most the roundings the bound already counts
     // (d accumulations of T, one subtraction).
     constexpr float kEps = 1.0f / 524288.0f;   // 2^-19
@@ -203,7 +198,7 @@ __device__ __forceinline__ void gnb_prepass_rows(const ScorerParams &P, const fl
 }
 
 // GATHER: the variant whose label stores go to every rank's peer-memory buffer (a separate instantiation: the plain kernel
-// must not pay for it -- with the code compiled in, the 1M-row step went from 10.5 to 11.3 us)
+// must not carry the path)
 template <typename T, int D, int R, int KIND, int kThreads, int kRPT, bool GATHER>
 __global__ void __launch_bounds__(kThreads) scorer_tiled_kernel(const __grid_constant__ ScorerParams P,
                                                                 const T *__restrict__ X, int64_t n,
@@ -236,8 +231,7 @@ __global__ void __launch_bounds__(kThreads) scorer_tiled_kernel(const __grid_con
     // Gathered mode: barrier A -- "every rank has entered this call", so nobody is still reading the previous vector -- is
     // ARRIVED at by one thread when the kernel starts and WAITED for by each CTA only before its first store into the peers:
     // the wait hides behind the first tile's load and scoring.  (Barrier B, "every rank's bytes are out", is a one-warp kernel
-    // behind this one: running it in the last CTA, with a system-scope fence in every CTA, measured slower, 29.7 against
-    // 23 us per step on two GPUs.)  Generations live in device memory: a CUDA graph holding the kernel can be replayed.
+    // behind this one, so that no CTA needs a system-scope fence.)  Generations live in device memory: a CUDA graph holding the kernel can be replayed.
     const bool fusedbar = GATHER && G.world && G.flags[0] != nullptr;
     unsigned genA = 0;
     bool a_passed = !fusedbar;
@@ -422,9 +416,8 @@ static int launch_tiled_cfg(tcsdn_model *m, const T *x, int64_t n, int32_t *labe
     int64_t n_tiles = (n + kTile - 1) / kTile;
     int64_t grid = (int64_t)m->sm_count * ctas_per_sm;
     if (grid > n_tiles) grid = n_tiles;
-    // (Programmatic dependent launch was tried here -- griddepcontrol.wait/launch_dependents with the PDL launch
-    // attribute -- and made the 1M-row CUDA-graph step slower, 15.1 vs 11.9 us: early-launched CTAs of the next grid
-    // sit on the SMs waiting.  Plain launches it is.)
+    // (Plain launches: with programmatic dependent launch, a correct griddepcontrol.wait has to precede the first load --
+    // the previous kernel may be the producer of X -- and early-launched CTAs of the next grid would sit on the SMs waiting.)
     // fp32 pre-pass: GaussianNB, float32 rows, labels only (TCSDN_OPT_ENGINE = 1 routes to the generic fp64 kernel instead)
     unsigned long long *refined = (KIND == KIND_GNB && sizeof(T) == 4 && scores == nullptr) ? m->d_refined : nullptr;
     kern<<<(unsigned)grid, kThreads, smem, st>>>(m->sp, x, n, labels, scores, flag, refined, G);
@@ -435,12 +428,11 @@ static int launch_tiled_cfg(tcsdn_model *m, const T *x, int64_t n, int32_t *labe
 template <typename T, int D, int R, int KIND>
 static int launch_tiled(tcsdn_model *m, const T *x, int64_t n, int32_t *labels, double *scores, int32_t *flag,
                         cudaStream_t st, const GatherOut &G) {
-    // CTA shape (measured on B200, 1M x 8 GaussianNB / 10M x 12 LogisticRegression, rows/s):
-    //   128 threads x 4 rows: 8.3e10 / 1.105e11    256 x 2: 7.9e10 / 1.132e11    256 x 4: 7.7e10 / 9.7e10    128 x 8: 8.3e10 / 7.7e10
-    // GaussianNB (fp64-pipe-bound) wants the constants amortised over 4 rows, the HBM-bound max/min scorers want more warps.
+    // CTA shape: GaussianNB wants the constants amortised over 4 rows (128 threads x 4), the HBM-bound max/min scorers want
+    // more warps (256 x 2).
     // Small batches: with 512-row tiles a 1M-row batch is 4.4 tiles per CTA -- the pipeline ramp (first tile) and the tail
     // (some CTAs own one tile more) are a quarter of the step -- so below 16 tiles per CTA the 256-row shape (128 x 2) is used.
-    // TCSDN_OPT_SCORER_SHAPE = 1 / 2 / 3 forces 128 x 4 / 256 x 2 / 128 x 2 (128 x 1 measured worse: 48 % against 53 %).
+    // TCSDN_OPT_SCORER_SHAPE = 1 / 2 / 3 forces 128 x 4 / 256 x 2 / 128 x 2.
     const int per_sm = sizeof(T) == 4 ? 3 : 2;
     int shape = (int)m->opt_scorer_shape;
     if (shape == 0) {

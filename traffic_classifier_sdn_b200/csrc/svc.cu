@@ -295,7 +295,7 @@ int launch_ovr_from_ovo(const double *dec, int64_t n, int C, double *out, cudaSt
     if (n == 0) return TCSDN_OK;
     if (C < 2 || C > kMaxClasses) { set_error("ovr_from_ovo: n_classes out of range"); return TCSDN_EINVAL; }
     int64_t blocks = (n + 127) / 128;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     ovr_from_ovo_kernel<<<(unsigned)blocks, 128, 0, st>>>(dec, n, C, out);
     TCSDN_CUDA(cudaGetLastError());
     return TCSDN_OK;

@@ -1,4 +1,4 @@
-"""sklearn-like estimators whose ``predict`` runs on the B200 through libtcsdn.so.
+"""sklearn-like estimators whose ``predict`` runs on the H100 through libtcsdn.so.
 
 These classes are the drop-in for the objects the reference gets from ``pickle.load`` at
 ``traffic_classifier.py:243`` and calls at ``traffic_classifier.py:106``
