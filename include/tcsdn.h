@@ -137,6 +137,19 @@ int tcsdn_model_stats(const tcsdn_model_t *m, int64_t *out);
 int tcsdn_predict(tcsdn_model_t *m, const void *x, int64_t n, int32_t d, int32_t x_dtype,
                   int32_t x_loc, int32_t *labels_out, double *scores_out, void *cuda_stream);
 
+/* KNeighborsClassifier.kneighbors(X, n_neighbors) (sk:neighbors/_base.py:750-960): per row of X the n_neighbors nearest
+ * training rows, ind_out [n][n_neighbors] int64 training indices and dist_out (nullable) [n][n_neighbors] float64
+ * euclidean distances, both where x_loc says.  The set is the one predict votes on: the rows sklearn's index-order heap
+ * keeps (ArgKmin, parallel_on_X; sk:utils/_heap.pyx), so with n_neighbors == k the vote of y[ind] is predict's label.
+ * Each row is in ascending (distance, training index) order -- sklearn leaves equal distances in no defined order, this
+ * call sorts them by index.  dist = sqrt(sum_f (x_f - t_f)^2), fp64, features in order, no FMA, correctly rounded sqrt;
+ * float32 rows are widened first.  1 <= n_neighbors <= min(64, n_samples_fit); TCSDN_EINVAL otherwise, for a handle that
+ * is not a KNeighborsClassifier and under engine options 3 and 4.  Path, device, counters ([1] engine rows, [2] fp64
+ * kernel rows, [7] index-order reruns) and non-finite rules are tcsdn_predict's: host pointers return TCSDN_ENONFINITE,
+ * device pointers set the sticky flag tcsdn_sync_check reads.  Host pointers are processed one chunk at a time. */
+int tcsdn_knn_kneighbors(tcsdn_model_t *m, const void *x, int64_t n, int32_t d, int32_t x_dtype, int32_t x_loc,
+                         int32_t n_neighbors, int64_t *ind_out, double *dist_out /* nullable */, void *cuda_stream);
+
 /* Host tail of `model.predict`: out[i] = table[idx[i]] for fixed-width class labels (numpy `classes_.take(idx)`,
  * sk:linear_model/_base.py:423), item_bytes bytes per label, gathered on up to n_threads host threads.  Host pointers. */
 int tcsdn_take_labels(const int32_t *idx, int64_t n, const void *table, int32_t n_items, int32_t item_bytes, void *out,

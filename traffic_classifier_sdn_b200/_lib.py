@@ -45,6 +45,7 @@ SIGNATURES = {
     "tcsdn_set_option": (C.c_int, [_vp, C.c_int32, C.c_int64]),
     "tcsdn_model_stats": (C.c_int, [_vp, _i64p]),
     "tcsdn_predict": (C.c_int, [_vp, _vp, C.c_int64, C.c_int32, C.c_int32, C.c_int32, _vp, _vp, _vp]),
+    "tcsdn_knn_kneighbors": (C.c_int, [_vp, _vp, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _vp, _vp, _vp]),
     "tcsdn_take_labels": (C.c_int, [_vp, C.c_int64, _vp, C.c_int32, C.c_int32, _vp, C.c_int32]),
     "tcsdn_sync_check": (C.c_int, [_vp, _vp]),
     "tcsdn_svc_ovr_from_ovo": (C.c_int, [_vp, C.c_int64, C.c_int32, C.c_int32, _vp, _vp]),

@@ -137,6 +137,15 @@ static int run_device(tcsdn_model *m, const void *x, int64_t n, int dtype, int32
     return TCSDN_EINVAL;
 }
 
+// kneighbors: the same choice of path as a knn predict (the engine keeps at most 32 neighbours per query)
+static int run_kneighbors(tcsdn_model *m, const void *x, int64_t n, int dtype, int nn, int64_t *ind, double *dist,
+                          int32_t *flag, cudaStream_t st) {
+    if (!m->opt_check_finite) flag = nullptr;
+    if (m->opt_engine != 1 && engine_kneighbors_usable(m, n, nn)) return launch_engine_kneighbors(m, x, n, dtype, nn, ind, dist, flag, st);
+    if (m->opt_engine == 2) { set_error("tensor-core engine forced but not usable for this model/batch/n_neighbors"); return TCSDN_EINVAL; }
+    return launch_knn_exact_kneighbors(m, x, n, dtype, nn, ind, dist, flag, st);
+}
+
 }  // namespace tcsdn
 
 using namespace tcsdn;
@@ -526,6 +535,81 @@ int tcsdn_predict(tcsdn_model_t *m, const void *x, int64_t n, int32_t d, int32_t
             }
         }
     } while (0);
+    release_workspace(m, w);
+    return rc;
+}
+
+int tcsdn_knn_kneighbors(tcsdn_model_t *m, const void *x, int64_t n, int32_t d, int32_t x_dtype, int32_t x_loc,
+                         int32_t n_neighbors, int64_t *ind_out, double *dist_out, void *cuda_stream) {
+    if (!m) { set_error("model is NULL"); return TCSDN_EINVAL; }
+    if (m->kind != TCSDN_KIND_KNN) { set_error("kneighbors needs a KNeighborsClassifier handle"); return TCSDN_EINVAL; }
+    if (n_neighbors < 1 || n_neighbors > 64 || n_neighbors > m->n_train) {
+        set_error("kneighbors: need 1 <= n_neighbors <= min(64, n_samples_fit), got n_neighbors=%d n_samples_fit=%lld", n_neighbors,
+                  (long long)m->n_train);
+        return TCSDN_EINVAL;
+    }
+    if (m->opt_engine >= 3) { set_error("kneighbors: engine options 3 and 4 are predict audits"); return TCSDN_EINVAL; }
+    if (n < 0) { set_error("n must be >= 0"); return TCSDN_EINVAL; }
+    if (d != m->d) {
+        set_error("X has %d features, but the model is expecting %d features as input", d, m->d);
+        return TCSDN_EINVAL;
+    }
+    if (x_dtype != TCSDN_F32 && x_dtype != TCSDN_F64) { set_error("x_dtype must be TCSDN_F32 or TCSDN_F64"); return TCSDN_EINVAL; }
+    if (x_loc != TCSDN_HOST && x_loc != TCSDN_DEVICE) { set_error("x_loc must be TCSDN_HOST or TCSDN_DEVICE"); return TCSDN_EINVAL; }
+    if (n == 0) return TCSDN_OK;
+    if (!x || !ind_out) { set_error("x / ind_out is NULL"); return TCSDN_EINVAL; }
+    struct DeviceGuard {
+        int prev = -1;
+        ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
+    } guard;
+    int cur = -1;
+    TCSDN_CUDA(cudaGetDevice(&cur));
+    if (cur != m->dev) { TCSDN_CUDA(cudaSetDevice(m->dev)); guard.prev = cur; }
+    for (int i = 0; i < 8; ++i) m->stats[i].store(0, std::memory_order_relaxed);
+    const int nn = n_neighbors;
+    if (x_loc == TCSDN_DEVICE)   // sticky non-finite flag, read by tcsdn_sync_check (as for tcsdn_predict)
+        return run_kneighbors(m, x, n, x_dtype, nn, ind_out, dist_out, m->d_flag, static_cast<cudaStream_t>(cuda_stream));
+
+    // host pointers: one chunk at a time on one internal stream (copy in, kernels, copy out, wait)
+    const size_t row_bytes = (size_t)d * (x_dtype == TCSDN_F32 ? 4 : 8);
+    const size_t out_row = (size_t)nn * sizeof(int64_t), dist_row = dist_out ? (size_t)nn * sizeof(double) : 0;
+    int64_t chunk = m->opt_chunk_rows;
+    if (chunk <= 0) {
+        chunk = (int64_t)((128u << 20) / (row_bytes + out_row + dist_row));
+        chunk = std::max<int64_t>(1024, (chunk / 1024) * 1024);
+    }
+    if (chunk > n) chunk = n;
+    Workspace *w = nullptr;
+    TCSDN_TRY(acquire_workspace(m, &w));
+    cudaStream_t st = w->stream[0];
+    int rc = ensure(w->x[0], (size_t)chunk * row_bytes);
+    if (rc == TCSDN_OK) rc = ensure(w->labels[0], (size_t)chunk * out_row);   // the workspace's label buffer holds ind here
+    if (rc == TCSDN_OK && dist_out) rc = ensure(w->scores[0], (size_t)chunk * dist_row);
+    if (rc == TCSDN_OK && m->opt_check_finite && cudaMemsetAsync(w->d_flag, 0, sizeof(int32_t), st) != cudaSuccess) {
+        set_error("flag reset failed");
+        rc = TCSDN_ECUDA;
+    }
+    for (int64_t done = 0; done < n && rc == TCSDN_OK;) {
+        const int64_t rows = std::min<int64_t>(chunk, n - done);
+        cudaError_t e = cudaMemcpyAsync(w->x[0].p, static_cast<const char *>(x) + (size_t)done * row_bytes, (size_t)rows * row_bytes,
+                                        cudaMemcpyHostToDevice, st);
+        if (e != cudaSuccess) { set_error("H2D copy failed: %s", cudaGetErrorString(e)); rc = TCSDN_ECUDA; break; }
+        rc = run_kneighbors(m, w->x[0].p, rows, x_dtype, nn, static_cast<int64_t *>(w->labels[0].p),
+                            dist_out ? static_cast<double *>(w->scores[0].p) : nullptr, w->d_flag, st);
+        if (rc != TCSDN_OK) break;
+        e = cudaMemcpyAsync(ind_out + (size_t)done * nn, w->labels[0].p, (size_t)rows * out_row, cudaMemcpyDeviceToHost, st);
+        if (e == cudaSuccess && dist_out)
+            e = cudaMemcpyAsync(dist_out + (size_t)done * nn, w->scores[0].p, (size_t)rows * dist_row, cudaMemcpyDeviceToHost, st);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+        if (e != cudaSuccess) { set_error("kneighbors failed: %s", cudaGetErrorString(e)); rc = TCSDN_ECUDA; break; }
+        done += rows;
+    }
+    if (rc != TCSDN_OK) cudaStreamSynchronize(st);   // nothing of this call may still run when the workspace is reused
+    if (rc == TCSDN_OK && m->opt_check_finite) {
+        cudaError_t e = cudaMemcpy(w->h_flag, w->d_flag, sizeof(int32_t), cudaMemcpyDeviceToHost);
+        if (e != cudaSuccess) { set_error("flag read failed: %s", cudaGetErrorString(e)); rc = TCSDN_ECUDA; }
+        else if (*w->h_flag) { set_error("Input X contains NaN or infinity"); rc = TCSDN_ENONFINITE; }
+    }
     release_workspace(m, w);
     return rc;
 }

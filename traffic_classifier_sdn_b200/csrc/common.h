@@ -88,6 +88,28 @@ __device__ __forceinline__ void peer_flag_wait(const GatherOut &G, int which, un
     }
 }
 
+// KNeighbors.kneighbors: one query's m kept neighbours (squared distance, training index), slot i at values[i * ST], sorted
+// in place into ascending (distance, index) order and written as one row of ind (and of dist = sqrt, correctly rounded, when
+// dist is non-null).  m <= 64: an insertion sort is all it needs.
+template <int ST>
+__device__ __forceinline__ void knn_write_neighbors(double *values, int32_t *indices, int m, int64_t *ind, double *dist) {
+    for (int i = 1; i < m; ++i) {
+        const double v = values[i * ST];
+        const int32_t x = indices[i * ST];
+        int j = i - 1;
+        for (; j >= 0 && (values[j * ST] > v || (values[j * ST] == v && indices[j * ST] > x)); --j) {
+            values[(j + 1) * ST] = values[j * ST];
+            indices[(j + 1) * ST] = indices[j * ST];
+        }
+        values[(j + 1) * ST] = v;
+        indices[(j + 1) * ST] = x;
+    }
+    for (int i = 0; i < m; ++i) {
+        ind[i] = indices[i * ST];
+        if (dist) dist[i] = __dsqrt_rn(values[i * ST]);
+    }
+}
+
 struct DeviceBuf {
     void *p = nullptr;
     size_t bytes = 0;
@@ -177,6 +199,12 @@ int launch_knn_exact(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_
 // the rows listed in list[0 .. *count) only (the knn engine's tie rows); *count is added to *total
 int launch_knn_marked(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, double *scores,
                       const int32_t *list, const int *count, unsigned long long *total, cudaStream_t st);
+// KNeighbors.kneighbors: per row the nn nearest training rows, ind [n][nn] int64 and dist [n][nn] (nullable), in
+// ascending (distance, index) order; the set is sklearn's index-order heap's, as for predict
+int launch_knn_exact_kneighbors(tcsdn_model *m, const void *x, int64_t n, int dtype, int nn, int64_t *ind, double *dist,
+                                int32_t *flag, cudaStream_t st);
+int launch_knn_marked_kneighbors(tcsdn_model *m, const void *x, int64_t n, int dtype, int nn, int64_t *ind, double *dist,
+                                 const int32_t *list, const int *count, unsigned long long *total, cudaStream_t st);
 int launch_svc_exact(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, double *scores,
                      int32_t *flag, cudaStream_t st);
 int launch_ovr_from_ovo(const double *dec, int64_t n, int C, double *out, cudaStream_t st);
@@ -197,6 +225,9 @@ int launch_svc_marked(tcsdn_model *m, const void *x, int64_t n, int dtype, int32
                       cudaStream_t st);
 int launch_engine(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, double *scores,
                   int32_t *flag, cudaStream_t st);
+bool engine_kneighbors_usable(const tcsdn_model *m, int64_t n, int nn);
+int launch_engine_kneighbors(tcsdn_model *m, const void *x, int64_t n, int dtype, int nn, int64_t *ind, double *dist,
+                             int32_t *flag, cudaStream_t st);
 
 template <typename T>
 int upload(T **dst, const T *src, size_t count) {

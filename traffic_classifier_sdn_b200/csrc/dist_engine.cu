@@ -27,6 +27,7 @@
 // k-th distance: there sklearn's answer depends on its heap's history.  The epilogue watches for rows left out at exactly the
 // final k-th distance; if such a row and the kept rows at that distance do not all carry one class, the query goes to the
 // index-order fp64 kernel (knn.cu, marked mode) in the same call; otherwise every choice gives the same class counts.
+// kneighbors (NC1 bit 2) returns the SET, so there any row left out at the final k-th distance sends the query to that kernel.
 // SVC uses acc directly, for LABELS only: e = -gamma log2(e) (acc + ||x' - c'_j||^2), K = ex2(e), C-1 fp32 FMAs per pair into
 // the running sums of the support vector's class, tile sums promoted to fp64.  To keep the fp32 accumulation error small
 // where K is not negligible, support vectors are re-ordered inside their class into spatially compact tiles and every tile
@@ -152,6 +153,7 @@ struct EngineState {
     uint16_t *d_nbr = nullptr;          // [n_tiles][n_tiles]: per home tile, all tiles by centre distance (nullptr: pruning off)
     float *d_chunk_lb = nullptr;        // [n_tiles][n_chunks]: min over positions >= 32 c of (centre distance - radius)
     int32_t *d_ypos = nullptr;          // training labels in tile order
+    int32_t *d_pos_orig = nullptr;      // KNN: tile position -> training index ([n_tiles * 64]; padding positions -1)
     float *d_tile_tn = nullptr;         // per tile: largest ||t - c0||^2 of its rows (rounded up)
     cudaMemPool_t pool = nullptr;       // per-call scratch (query keys, permutation, tie list): stream-ordered allocations
     int n_tiles = 0;
@@ -191,6 +193,11 @@ struct EngineArgs {
     float g2;                // SVC: -gamma * log2(e)
     float svc_c1, svc_c2;    // SVC: gamma (2^-20 + 2^-24) and gamma 2^-24, the row-dependent parts of eta_j
     float svc_eabs[(kEMaxNC1 + 1) * kEMaxNC1 / 2];   // SVC: per pair, the absolute part of E_p (file header)
+    // KNN kneighbors instantiations (NC1 bit 2): k is the call's n_neighbors; per row, the kept training indices (int64) and,
+    // when nb_dist is non-null, their distances, [n][k] in ascending (distance, index) order
+    const int32_t *pos_orig; // tile position -> training index
+    int64_t *nb_ind;
+    double *nb_dist;
 };
 
 // ------------------------------------------------------------------------------------------------ PTX helpers
@@ -742,7 +749,8 @@ engine_kernel(const __grid_constant__ EngineArgs A, const T *__restrict__ X, int
                 // The k-slot max-heap: shared memory [slot][thread] for k <= 8 (NC1 bit 0), else thread-private local
                 // memory.  Its root and the filter threshold stay in registers.
                 constexpr bool kHeapSmem = (NC1 & 1) != 0;      // KNN instantiations: NC1 bit 0 = heap in shared memory,
-                constexpr bool kAudit = (NC1 & 2) != 0;         //                     bit 1 = audit mode (error statistic)
+                constexpr bool kAudit = (NC1 & 2) != 0;         //                     bit 1 = audit mode (error statistic),
+                constexpr bool kKnb = (NC1 & 4) != 0;           //                     bit 2 = kneighbors (rows of A.nb_ind / A.nb_dist)
                 constexpr int ST = kHeapSmem ? kKnnRows : 1;
                 double hv_local[kHeapSmem ? 1 : kEMaxK];
                 int32_t hi_local[kHeapSmem ? 1 : kEMaxK];
@@ -950,15 +958,20 @@ engine_kernel(const __grid_constant__ EngineArgs A, const T *__restrict__ X, int
                 }
                 KT_START();
                 if (live) {
-                    // a row outside the kept set at exactly the k-th distance: does the choice among the tied rows matter?
+                    // a row outside the kept set at exactly the k-th distance: does the choice among the tied rows matter?  For
+                    // the vote only if the tied rows' classes differ; for kneighbors always (the SET is the index-order heap's)
                     bool tied = false;
                     if (tie_val == hv0) {
-                        tied = tie_cls < 0;
-                        for (int i = 0; i < A.k; ++i) tied |= (hv[i * ST] == hv0 && A.ypos[hi[i * ST]] != tie_cls);
+                        tied = kKnb || tie_cls < 0;
+                        if constexpr (!kKnb)
+                            for (int i = 0; i < A.k; ++i) tied |= (hv[i * ST] == hv0 && A.ypos[hi[i * ST]] != tie_cls);
                     }
                     if (tied) {
-                        labels[row] = -1;
+                        if constexpr (!kKnb) labels[row] = -1;
                         A.tie_list[atomicAdd(A.tie_count, 1)] = (int32_t)row;
+                    } else if constexpr (kKnb) {
+                        for (int i = 0; i < A.k; ++i) hi[i * ST] = A.pos_orig[hi[i * ST]];
+                        knn_write_neighbors<ST>(hv, hi, A.k, A.nb_ind + row * A.k, A.nb_dist ? A.nb_dist + row * A.k : nullptr);
                     } else {
                         int best = 0, arg = 0;
                         for (int c = 0; c < A.C; ++c) {
@@ -1529,14 +1542,16 @@ int engine_create(tcsdn_model *m) {
         const int dpad = kEMaxD;
         const size_t npos = (size_t)E->n_tiles * kEN;
         std::vector<double> pad(npos * dpad, 0.0);
-        std::vector<int32_t> ypos(npos, 0), yh((size_t)nref);
+        std::vector<int32_t> ypos(npos, 0), yh((size_t)nref), pos_orig(npos, -1);
         TCSDN_CUDA(cudaMemcpy(yh.data(), m->d_y, yh.size() * sizeof(int32_t), cudaMemcpyDeviceToHost));
         for (int64_t i = 0; i < nref; ++i) {
             memcpy(&pad[(size_t)i * dpad], &ref[(size_t)order[(size_t)i] * d], (size_t)d * sizeof(double));
             ypos[(size_t)i] = yh[(size_t)order[(size_t)i]];
+            pos_orig[(size_t)i] = order[(size_t)i];
         }
         rc = upload(&E->d_refpad, pad.data(), pad.size());
         if (rc == TCSDN_OK) rc = upload(&E->d_ypos, ypos.data(), ypos.size());
+        if (rc == TCSDN_OK) rc = upload(&E->d_pos_orig, pos_orig.data(), pos_orig.size());
         if (rc == TCSDN_OK) rc = upload(&E->d_tile_tn, tile_tn.data(), tile_tn.size());
         // pruning tables: tile centres and radii, the kd tree, and per home tile the tiles by centre distance
         const int nt = E->n_tiles;
@@ -1614,7 +1629,7 @@ void engine_destroy(tcsdn_model *m) {
     cudaFree(E->d_tiles); cudaFree(E->d_tile_class); cudaFree(E->d_tile_row0); cudaFree(E->d_tile_rows);
     cudaFree(E->d_center); cudaFree(E->d_refpad); cudaFree(E->d_maxratio); cudaFree(E->d_counters);
     cudaFree(E->d_kd_dim); cudaFree(E->d_kd_child); cudaFree(E->d_kd_split); cudaFree(E->d_leaf_tile); cudaFree(E->d_tcent); cudaFree(E->d_trad);
-    cudaFree(E->d_nbr); cudaFree(E->d_chunk_lb); cudaFree(E->d_ypos); cudaFree(E->d_tile_tn);
+    cudaFree(E->d_nbr); cudaFree(E->d_chunk_lb); cudaFree(E->d_ypos); cudaFree(E->d_tile_tn); cudaFree(E->d_pos_orig);
     if (E->pool) cudaMemPoolDestroy(E->pool);
     delete E;
     m->engine = nullptr;
@@ -1631,9 +1646,11 @@ bool engine_usable(const tcsdn_model *m, int64_t n, bool want_scores) {
     return n >= 4096;   // below this the fp64 CUDA-core kernels (latency path) are faster than filling every SM with 256-row passes
 }
 
+// kk: neighbours kept per query (KNN: the model's k for predict, the call's n_neighbors for kneighbors); nb_ind non-null
+// selects the kneighbors instantiations, which write nb_ind / nb_dist instead of labels / scores
 template <typename T>
 static int launch_engine_t(tcsdn_model *m, const T *x, int64_t n, int32_t *labels, double *scores, int32_t *flag,
-                           cudaStream_t st) {
+                           cudaStream_t st, int kk, int64_t *nb_ind, double *nb_dist) {
     EngineState *E = static_cast<EngineState *>(m->engine);
     const bool svc = m->kind == TCSDN_KIND_SVC;
     EngineArgs A;
@@ -1643,7 +1660,8 @@ static int launch_engine_t(tcsdn_model *m, const T *x, int64_t n, int32_t *label
     // largest |tensor-core value - exact| / (error model's denominator) is recorded (stats[5]); tests only
     A.maxratio = m->opt_engine == 3 ? E->d_maxratio : nullptr;
     A.flag = flag; A.n = n; A.n_tiles = E->n_tiles;
-    A.tile_bytes = E->tile_bytes; A.d = m->d; A.k = m->k; A.C = m->n_classes; A.nc1 = E->nc1;
+    A.tile_bytes = E->tile_bytes; A.d = m->d; A.k = kk; A.C = m->n_classes; A.nc1 = E->nc1;
+    A.pos_orig = E->d_pos_orig; A.nb_ind = nb_ind; A.nb_dist = nb_dist;
     A.refpad = E->d_refpad; A.dpad = kEMaxD;
     A.flush_tiles = m->opt_knn_flush > 0 ? (int)m->opt_knn_flush : kEFlushTiles;   // TCSDN_OPT_KNN_FLUSH_TILES
     A.n_ref = (int)(svc ? m->n_sv : m->n_train);
@@ -1652,7 +1670,7 @@ static int launch_engine_t(tcsdn_model *m, const T *x, int64_t n, int32_t *label
     A.svc_c1 = std::nextafterf(static_cast<float>(m->gamma * (1.0 / 1048576.0 + 1.0 / 16777216.0)), INFINITY);
     A.svc_c2 = std::nextafterf(static_cast<float>(m->gamma / 16777216.0), INFINITY);
     for (int p = 0; p < (kEMaxNC1 + 1) * kEMaxNC1 / 2; ++p) A.svc_eabs[p] = E->eabs[p];
-    const bool heap_smem = !svc && m->k <= kEHeapSmemK;
+    const bool heap_smem = !svc && kk <= kEHeapSmemK;
     const int P = m->n_classes * (m->n_classes - 1) / 2;
     // KNN: order the queries by home tile (counting sort on this stream) so that a pass's 256 rows are neighbours and the
     // producer can leave out the tiles that are too far for all of them.  Scratch comes from the engine's own stream-ordered
@@ -1698,7 +1716,7 @@ static int launch_engine_t(tcsdn_model *m, const T *x, int64_t n, int32_t *label
     const int rows_per_pass = svc ? kERows : kKnnRows;
     const size_t smem = (size_t)(rows_per_pass / 128) * kEATile + kETBytes + (size_t)kEStages * E->tile_bytes + kEBarRegion +
                         (svc ? (size_t)P * kERows * (sizeof(double) + sizeof(float))
-                             : kKnnRows * (size_t)kEListCap * sizeof(uint16_t) + (heap_smem ? kKnnRows * (size_t)m->k * 12 : 0));
+                             : kKnnRows * (size_t)kEListCap * sizeof(uint16_t) + (heap_smem ? kKnnRows * (size_t)kk * 12 : 0));
     const int64_t n_super = (n + rows_per_pass - 1) / rows_per_pass;
     const unsigned grid = (unsigned)std::min<int64_t>(n_super, (int64_t)m->sm_count);
 #define TCSDN_LAUNCH(SVCF, NC)                                                                                    \
@@ -1708,12 +1726,15 @@ static int launch_engine_t(tcsdn_model *m, const T *x, int64_t n, int32_t *label
         kern<<<grid, SVCF ? kESvcThreads : kEKnnThreads, smem, st>>>(A, x, labels, scores, E->d_counters);        \
     }
     if (!svc) {
-        const int variant = (heap_smem ? 1 : 0) | (A.maxratio ? 2 : 0);
+        const int variant = (heap_smem ? 1 : 0) | (A.maxratio ? 2 : 0) | (nb_ind ? 4 : 0);
         switch (variant) {
             case 0: TCSDN_LAUNCH(false, 0) break;
             case 1: TCSDN_LAUNCH(false, 1) break;
             case 2: TCSDN_LAUNCH(false, 2) break;
-            default: TCSDN_LAUNCH(false, 3) break;
+            case 3: TCSDN_LAUNCH(false, 3) break;
+            case 4: TCSDN_LAUNCH(false, 4) break;
+            case 5: TCSDN_LAUNCH(false, 5) break;
+            default: set_error("knn engine: kneighbors has no audit mode"); return TCSDN_EINVAL;
         }
     }
     else switch (E->nc1) {
@@ -1730,6 +1751,9 @@ static int launch_engine_t(tcsdn_model *m, const T *x, int64_t n, int32_t *label
     m->stats[1] += n;
     // SVC: rows the certificate could not decide carry -1 - label; the fp64 kernel re-evaluates exactly those (same stream)
     if (svc && A.svc_mode == 0) return launch_svc_marked(m, x, n, sizeof(T) == 4 ? TCSDN_F32 : TCSDN_F64, labels, E->d_counters, st);
+    if (!svc && nb_ind)   // kneighbors: rows whose neighbour SET hangs on a tie at the k-th distance, likewise
+        return launch_knn_marked_kneighbors(m, x, n, sizeof(T) == 4 ? TCSDN_F32 : TCSDN_F64, kk, nb_ind, nb_dist, A.tie_list,
+                                            A.tie_count, E->d_counters + 1, st);
     if (!svc) {   // KNN: rows whose label hangs on a tie at the k-th distance get sklearn's index-order heap (knn.cu)
         return launch_knn_marked(m, x, n, sizeof(T) == 4 ? TCSDN_F32 : TCSDN_F64, labels, scores, A.tie_list, A.tie_count,
                                  E->d_counters + 1, st);
@@ -1740,8 +1764,19 @@ static int launch_engine_t(tcsdn_model *m, const T *x, int64_t n, int32_t *label
 int launch_engine(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, double *scores, int32_t *flag,
                   cudaStream_t st) {
     if (n == 0) return TCSDN_OK;
-    if (dtype == TCSDN_F32) return launch_engine_t<float>(m, static_cast<const float *>(x), n, labels, scores, flag, st);
-    return launch_engine_t<double>(m, static_cast<const double *>(x), n, labels, scores, flag, st);
+    if (dtype == TCSDN_F32) return launch_engine_t<float>(m, static_cast<const float *>(x), n, labels, scores, flag, st, m->k, nullptr, nullptr);
+    return launch_engine_t<double>(m, static_cast<const double *>(x), n, labels, scores, flag, st, m->k, nullptr, nullptr);
+}
+
+bool engine_kneighbors_usable(const tcsdn_model *m, int64_t n, int nn) {
+    return m->kind == TCSDN_KIND_KNN && nn <= kEMaxK && engine_usable(m, n, false);
+}
+
+int launch_engine_kneighbors(tcsdn_model *m, const void *x, int64_t n, int dtype, int nn, int64_t *ind, double *dist,
+                             int32_t *flag, cudaStream_t st) {
+    if (n == 0) return TCSDN_OK;
+    if (dtype == TCSDN_F32) return launch_engine_t<float>(m, static_cast<const float *>(x), n, nullptr, nullptr, flag, st, nn, ind, dist);
+    return launch_engine_t<double>(m, static_cast<const double *>(x), n, nullptr, nullptr, flag, st, nn, ind, dist);
 }
 
 // cumulative engine counters since create() (synchronising read): out[3] exact re-evaluations of the knn filter,

@@ -10,7 +10,8 @@
 // for small batches (the reference's own call is one row at a time, traffic_classifier.py:106), as the
 // engine's exact re-evaluation rule, and as the engine's cross-check in the tests.  One thread owns one
 // query and scans the training rows in index order out of a shared-memory tile (all lanes read the same
-// training row: broadcast), so the heap sees exactly sklearn's push sequence.
+// training row: broadcast), so the heap sees exactly sklearn's push sequence.  Both kernels have a kneighbors mode (template
+// flag KNB): the same heap, then the kept rows in ascending (distance, index) order instead of the vote.
 #include <cfloat>
 
 #include "common.h"
@@ -44,12 +45,15 @@ __device__ __forceinline__ void heap_push_dev(double *values, int32_t *indices, 
     indices[cur] = val_idx;
 }
 
-template <typename T>
+// KNB (kneighbors): instead of the vote, the k kept rows in ascending (distance, index) order go to nb_ind / nb_dist
+// [n][k] (nb_dist nullable); labels and proba are unused.  The predict instantiation ignores the two trailing arguments.
+template <typename T, bool KNB = false>
 __global__ void __launch_bounds__(kKnnThreads) knn_exact_kernel(const T *__restrict__ X, int64_t n, int d,
                                                                 const double *__restrict__ fit,
                                                                 const int32_t *__restrict__ y, int64_t n_train,
                                                                 int k, int C, int32_t *__restrict__ labels,
-                                                                double *__restrict__ proba, int32_t *flag) {
+                                                                double *__restrict__ proba, int32_t *flag,
+                                                                int64_t *__restrict__ nb_ind, double *__restrict__ nb_dist) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     double *qs = reinterpret_cast<double *>(smem_raw);           // [d][kKnnThreads]
     double *ts = qs + (size_t)d * kKnnThreads;                   // [kKnnTile][d]
@@ -85,7 +89,9 @@ __global__ void __launch_bounds__(kKnnThreads) knn_exact_kernel(const T *__restr
                 }
             }
         }
-        if (live) {
+        if constexpr (KNB) {
+            if (live) knn_write_neighbors<1>(hv, hi, k, nb_ind + q * k, nb_dist ? nb_dist + q * k : nullptr);
+        } else if (live) {
             int best = 0, arg = 0;
             for (int c = 0; c < C; ++c) {
                 int cnt = 0;
@@ -99,8 +105,10 @@ __global__ void __launch_bounds__(kKnnThreads) knn_exact_kernel(const T *__restr
     if (flag && nf != nf) atomicOr(flag, 1);
 }
 
-int launch_knn_exact(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, double *scores,
-                     int32_t *flag, cudaStream_t st) {
+// predict (nb_ind == nullptr: labels / scores, the model's k) or kneighbors (nb_ind / nb_dist, k = the call's n_neighbors)
+template <bool KNB>
+static int launch_exact(tcsdn_model *m, const void *x, int64_t n, int dtype, int k, int32_t *labels, double *scores,
+                        int64_t *nb_ind, double *nb_dist, int32_t *flag, cudaStream_t st) {
     if (n == 0) return TCSDN_OK;
     const size_t smem = ((size_t)m->d * kKnnThreads + (size_t)kKnnTile * m->d) * sizeof(double);
     int64_t blocks = (n + kKnnThreads - 1) / kKnnThreads;
@@ -109,18 +117,28 @@ int launch_knn_exact(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_
     m->stats[0] += 1;
     m->stats[2] += n;
     if (dtype == TCSDN_F32) {
-        auto kern = knn_exact_kernel<float>;
+        auto kern = knn_exact_kernel<float, KNB>;
         TCSDN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kern<<<(unsigned)blocks, kKnnThreads, smem, st>>>(static_cast<const float *>(x), n, m->d, m->d_fit, m->d_y,
-                                                          m->n_train, m->k, m->n_classes, labels, scores, flag);
+                                                          m->n_train, k, m->n_classes, labels, scores, flag, nb_ind, nb_dist);
     } else {
-        auto kern = knn_exact_kernel<double>;
+        auto kern = knn_exact_kernel<double, KNB>;
         TCSDN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kern<<<(unsigned)blocks, kKnnThreads, smem, st>>>(static_cast<const double *>(x), n, m->d, m->d_fit, m->d_y,
-                                                          m->n_train, m->k, m->n_classes, labels, scores, flag);
+                                                          m->n_train, k, m->n_classes, labels, scores, flag, nb_ind, nb_dist);
     }
     TCSDN_CUDA(cudaGetLastError());
     return TCSDN_OK;
+}
+
+int launch_knn_exact(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, double *scores,
+                     int32_t *flag, cudaStream_t st) {
+    return launch_exact<false>(m, x, n, dtype, m->k, labels, scores, nullptr, nullptr, flag, st);
+}
+
+int launch_knn_exact_kneighbors(tcsdn_model *m, const void *x, int64_t n, int dtype, int nn, int64_t *ind, double *dist,
+                                int32_t *flag, cudaStream_t st) {
+    return launch_exact<true>(m, x, n, dtype, nn, nullptr, nullptr, ind, dist, flag, st);
 }
 
 // The tensor-core engine's tie rows (dist_engine.cu): a few rows per ten thousand whose label depends on which of several
@@ -129,12 +147,14 @@ int launch_knn_exact(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_
 // in step -- the sequential heap's result at 1/32 of its latency.  The number of rows is only known on the device.
 constexpr int kTieMaxD = 12;   // the engine's feature limit
 
-template <typename T>
+// KNB (kneighbors): lane 0 writes the k kept rows in ascending (distance, index) order to nb_ind / nb_dist instead of the vote
+template <typename T, bool KNB = false>
 __global__ void __launch_bounds__(256) knn_tie_kernel(const T *__restrict__ X, int d, const double *__restrict__ fit,
                                                       const int32_t *__restrict__ y, int64_t n_train, int k, int C,
                                                       int32_t *__restrict__ labels, double *__restrict__ proba,
                                                       const int32_t *__restrict__ list, const int *__restrict__ n_list,
-                                                      unsigned long long *total) {
+                                                      unsigned long long *total, int64_t *__restrict__ nb_ind,
+                                                      double *__restrict__ nb_dist) {
     const int n = *n_list;
     if (total && blockIdx.x == 0 && threadIdx.x == 0 && n > 0) atomicAdd(total, (unsigned long long)n);
     const int lane = threadIdx.x & 31;
@@ -178,7 +198,9 @@ __global__ void __launch_bounds__(256) knn_tie_kernel(const T *__restrict__ X, i
                 }
             }
         }
-        if (lane == 0) {
+        if constexpr (KNB) {
+            if (lane == 0) knn_write_neighbors<1>(hv, hi, k, nb_ind + q * k, nb_dist ? nb_dist + q * k : nullptr);
+        } else if (lane == 0) {
             int best = 0, arg = 0;
             for (int c = 0; c < C; ++c) {
                 int cnt = 0;
@@ -191,8 +213,10 @@ __global__ void __launch_bounds__(256) knn_tie_kernel(const T *__restrict__ X, i
     }
 }
 
-int launch_knn_marked(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, double *scores,
-                      const int32_t *list, const int *count, unsigned long long *total, cudaStream_t st) {
+template <bool KNB>
+static int launch_marked(tcsdn_model *m, const void *x, int64_t n, int dtype, int k, int32_t *labels, double *scores,
+                         int64_t *nb_ind, double *nb_dist, const int32_t *list, const int *count, unsigned long long *total,
+                         cudaStream_t st) {
     if (n == 0) return TCSDN_OK;
     if (m->d > kTieMaxD) { set_error("knn tie kernel: more than %d features", kTieMaxD); return TCSDN_EINVAL; }
     int64_t blocks = (n + 7) / 8;                     // eight rows (warps) per block
@@ -200,13 +224,23 @@ int launch_knn_marked(tcsdn_model *m, const void *x, int64_t n, int dtype, int32
     if (blocks > cap) blocks = cap;
     m->stats[0] += 1;
     if (dtype == TCSDN_F32)
-        knn_tie_kernel<float><<<(unsigned)blocks, 256, 0, st>>>(static_cast<const float *>(x), m->d, m->d_fit, m->d_y, m->n_train, m->k,
-                                                                m->n_classes, labels, scores, list, count, total);
+        knn_tie_kernel<float, KNB><<<(unsigned)blocks, 256, 0, st>>>(static_cast<const float *>(x), m->d, m->d_fit, m->d_y, m->n_train,
+                                                                     k, m->n_classes, labels, scores, list, count, total, nb_ind, nb_dist);
     else
-        knn_tie_kernel<double><<<(unsigned)blocks, 256, 0, st>>>(static_cast<const double *>(x), m->d, m->d_fit, m->d_y, m->n_train, m->k,
-                                                                 m->n_classes, labels, scores, list, count, total);
+        knn_tie_kernel<double, KNB><<<(unsigned)blocks, 256, 0, st>>>(static_cast<const double *>(x), m->d, m->d_fit, m->d_y, m->n_train,
+                                                                      k, m->n_classes, labels, scores, list, count, total, nb_ind, nb_dist);
     TCSDN_CUDA(cudaGetLastError());
     return TCSDN_OK;
+}
+
+int launch_knn_marked(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, double *scores,
+                      const int32_t *list, const int *count, unsigned long long *total, cudaStream_t st) {
+    return launch_marked<false>(m, x, n, dtype, m->k, labels, scores, nullptr, nullptr, list, count, total, st);
+}
+
+int launch_knn_marked_kneighbors(tcsdn_model *m, const void *x, int64_t n, int dtype, int nn, int64_t *ind, double *dist,
+                                 const int32_t *list, const int *count, unsigned long long *total, cudaStream_t st) {
+    return launch_marked<true>(m, x, n, dtype, nn, nullptr, nullptr, ind, dist, list, count, total, st);
 }
 
 }  // namespace tcsdn

@@ -8,6 +8,7 @@ These classes are the drop-in for the objects the reference gets from ``pickle.l
   KMeans); ``classes_``, ``n_features_in_``; ``decision_function`` (LogisticRegression, SVC),
   ``predict_proba`` (GaussianNB, KNeighborsClassifier, RandomForestClassifier), ``predict_log_proba`` /
   ``transform`` where sklearn has them and they are a closed form of the kernel's score matrix;
+  ``kneighbors`` (KNeighborsClassifier);
 * ``ValueError`` on a wrong feature count or NaN/inf input, ``NotFittedError`` before ``fit``;
   inputs are never modified, outputs are freshly allocated.
 
@@ -444,6 +445,84 @@ class KNeighborsClassifier(_Base):
 
     def predict_proba(self, X):
         return self._scores(X)
+
+    def kneighbors(self, X=None, n_neighbors=None, return_distance=True):
+        """sk:neighbors/_base.py:750-960 -- the n_neighbors nearest training rows of every row of X: ``(dist, ind)`` (float64,
+        int64, [n, n_neighbors]), or ``ind`` alone.  The neighbours are the ones ``predict`` votes on (sklearn's index-order
+        heap); each row is sorted by (distance, training index), where sklearn leaves equal distances in no defined order.
+        ``X=None`` queries the training rows and leaves each row's own index out (sklearn's rule).  A CUDA ``torch.Tensor``
+        gives CUDA tensors, enqueued on the current stream (``sync_check()`` reports NaN/inf rows).  At most 64 neighbours
+        (63 with ``X=None``)."""
+        import numbers
+        self._check_fitted()
+        if n_neighbors is None:
+            n_neighbors = int(self._spec["k"])
+        elif n_neighbors <= 0:
+            raise ValueError("Expected n_neighbors > 0. Got %d" % n_neighbors)
+        elif not isinstance(n_neighbors, numbers.Integral):
+            raise TypeError("n_neighbors does not take %s value, enter integer value" % type(n_neighbors))
+        n_neighbors = int(n_neighbors)
+        query_is_train = X is None
+        if query_is_train:
+            X = np.ascontiguousarray(self._spec["fit_X"], np.float64)
+            n_neighbors += 1                         # the row itself comes back too and is removed below
+        X, n, d, dt, loc = self._query_rows(X)
+        if d != self.n_features_in_:
+            raise ValueError(f"X has {d} features, but {type(self).__name__} is expecting {self.n_features_in_} features as input")
+        if n_neighbors > self.n_samples_fit_:
+            if query_is_train:
+                n_neighbors -= 1
+                inequality = "n_neighbors < n_samples_fit"
+            else:
+                inequality = "n_neighbors <= n_samples_fit"
+            raise ValueError(f"Expected {inequality}, but n_neighbors = {n_neighbors}, n_samples_fit = {self.n_samples_fit_}, "
+                             f"n_samples = {n}")
+        if n_neighbors > 64:
+            raise ValueError(f"kneighbors keeps at most 64 neighbours per row (with X=None: 63), got n_neighbors = "
+                             f"{n_neighbors - 1 if query_is_train else n_neighbors}")
+        lib = _lib.load()
+        if loc == _lib.DEVICE:
+            import torch
+            ind = torch.empty((n, n_neighbors), dtype=torch.int64, device=X.device)
+            dist = torch.empty((n, n_neighbors), dtype=torch.float64, device=X.device) if return_distance else None
+            with torch.cuda.device(X.device):
+                st = torch.cuda.current_stream().cuda_stream
+                _lib.check(lib.tcsdn_knn_kneighbors(self._handle, X.data_ptr(), n, d, dt, loc, n_neighbors, ind.data_ptr(),
+                                                    dist.data_ptr() if return_distance else None, st))
+            return (dist, ind) if return_distance else ind
+        ind = np.empty((n, n_neighbors), np.int64)
+        dist = np.empty((n, n_neighbors), np.float64) if return_distance else None
+        _lib.check(lib.tcsdn_knn_kneighbors(self._handle, _lib.ptr(X), n, d, dt, loc, n_neighbors, _lib.ptr(ind),
+                                            _lib.ptr(dist) if return_distance else None, None))
+        if query_is_train:
+            # sk:neighbors/_base.py:930-956: drop each row's own index; where more duplicates than neighbours push it out
+            # of the n_neighbors + 1 kept rows, drop the first column instead
+            keep = ind != np.arange(n)[:, None]
+            keep[np.all(keep, axis=1), 0] = False
+            ind = ind[keep].reshape(n, n_neighbors - 1)
+            if return_distance:
+                dist = dist[keep].reshape(n, n_neighbors - 1)
+        return (dist, ind) if return_distance else ind
+
+    @staticmethod
+    def _query_rows(X):
+        """-> (rows, n, d, dtype code, loc code) for a query: a contiguous float32/float64 CUDA tensor or numpy array
+        (other dtypes are widened to float64, as predict does)."""
+        if _is_torch_cuda(X):
+            import torch
+            if X.dim() != 2:
+                raise ValueError(f"Expected 2D array, got {X.dim()}D tensor instead")
+            if X.dtype not in (torch.float32, torch.float64):
+                X = X.to(torch.float64)
+            X = X.contiguous()
+            return X, X.shape[0], X.shape[1], _lib.F32 if X.dtype == torch.float32 else _lib.F64, _lib.DEVICE
+        A = X if isinstance(X, np.ndarray) else np.asarray(X)
+        if A.ndim != 2:
+            raise ValueError(f"Expected 2D array, got {A.ndim}D array instead")
+        if A.dtype not in (np.float32, np.float64):
+            A = A.astype(np.float64)
+        A = np.ascontiguousarray(A)
+        return A, A.shape[0], A.shape[1], _lib.F32 if A.dtype == np.float32 else _lib.F64, _lib.HOST
 
 
 class SVC(_Base):
