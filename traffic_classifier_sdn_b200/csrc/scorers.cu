@@ -282,6 +282,18 @@ __global__ void __launch_bounds__(kThreads) scorer_tiled_kernel(const __grid_con
     }
 
     float nf = 0.f;
+    // Every thread has lifted its rows out of the stage: refill it with the tile kStages rounds ahead.  The bulk copy (async
+    // proxy) must not overtake shared loads that are still in flight, and neither BAR.SYNC nor a MEMBAR.CTA in front of it
+    // waits for those (see dist_engine.cu for the hazard): the fp32 pre-pass, whose loaded values are consumed only after the
+    // barrier, got rows of the NEXT tile from the refilled stage.  So the barrier's predicate is nf, which depends on every
+    // value this thread loaded: the barrier cannot complete before all loads of the CTA have returned.
+    auto release = [&](int64_t tile, int stage) {
+        if (__syncthreads_or(nf != nf) && flag && tid == 0) atomicOr(flag, 1);
+        if (tid == 0) {
+            int64_t nt = tile + (int64_t)kStages * stride;
+            if (nt < n_tiles) issue(nt, stage);
+        }
+    };
     int it = 0;
     for (int64_t tile = first; tile < n_tiles; tile += stride, ++it) {
         const int stage = it % kStages;
@@ -303,19 +315,16 @@ __global__ void __launch_bounds__(kThreads) scorer_tiled_kernel(const __grid_con
                         nf = fmaf(u.x, 0.f, nf); nf = fmaf(u.y, 0.f, nf); nf = fmaf(u.z, 0.f, nf); nf = fmaf(u.w, 0.f, nf);
                     }
                 }
-                __threadfence_block();
-                __syncthreads();
-                if (tid == 0) {
-                    int64_t nt = tile + (int64_t)kStages * stride;
-                    if (nt < n_tiles) issue(nt, stage);
-                }
+                release(tile, stage);
                 int arg[kRPT];
                 bool sure[kRPT];
                 gnb_prepass_rows<D, R, kRPT>(P, xf, arg, sure);
                 unsigned redo = 0;
 #pragma unroll
                 for (int q = 0; q < kRPT; ++q) {
-                    if (!sure[q]) {   // rare: this row's top-2 margin is inside the fp32 error bound -> the fp64 definition decides
+                    // rare: this row's top-2 margin is inside the fp32 error bound -> the fp64 definition decides (the zero
+                    // padding past n in the last tile is neither re-run nor counted)
+                    if (!sure[q] && row0 + q * kThreads + tid < n) {
                         double xd[1][D], s1[1][R];
                         int a1[1];
 #pragma unroll
@@ -339,15 +348,7 @@ __global__ void __launch_bounds__(kThreads) scorer_tiled_kernel(const __grid_con
                 for (int j = 0; j < D; ++j) x[q][j] = 0.0;
             }
         }
-        // The stage is refilled by the async proxy (bulk copy) right after this barrier.  BAR.SYNC orders generic-proxy
-        // accesses among threads, but the bulk copy must not overtake shared loads that are still in flight, so every
-        // thread first makes sure its loads have been performed (MEMBAR.CTA; see dist_engine.cu for the hazard).
-        __threadfence_block();
-        __syncthreads();  // every thread has lifted its rows: the stage may be refilled
-        if (tid == 0) {
-            int64_t nt = tile + (int64_t)kStages * stride;
-            if (nt < n_tiles) issue(nt, stage);
-        }
+        release(tile, stage);
         double s[kRPT][R];
         int arg[kRPT];
         score_rows<D, R, KIND, kRPT>(P, x, s, arg);
@@ -408,10 +409,15 @@ static int launch_tiled_cfg(tcsdn_model *m, const T *x, int64_t n, int32_t *labe
     auto kern = (kCanGather && G.world) ? scorer_tiled_kernel<T, D, R, KIND, kThreads, kRPT, kCanGather>
                                         : scorer_tiled_kernel<T, D, R, KIND, kThreads, kRPT, false>;
     const size_t smem = (size_t)kStages * kTile * D * sizeof(T) + kStages * sizeof(uint64_t);
-    static bool configured[2] = {false, false};  // per instantiation and variant
-    if (!configured[G.world ? 1 : 0]) {
+    // The opt-in above 48 KB is an attribute of the kernel on the current device: it is made once per device (one bit per
+    // device ordinal, per instantiation and variant), so that a process predicting on several GPUs opts in on each of them.
+    static std::atomic<uint64_t> configured[2] = {};
+    int dev = 0;
+    TCSDN_CUDA(cudaGetDevice(&dev));
+    const uint64_t dev_bit = dev < 64 ? (uint64_t)1 << dev : 0;
+    if (!(configured[G.world ? 1 : 0].load(std::memory_order_relaxed) & dev_bit)) {
         TCSDN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        configured[G.world ? 1 : 0] = true;
+        configured[G.world ? 1 : 0].fetch_or(dev_bit, std::memory_order_relaxed);
     }
     int64_t n_tiles = (n + kTile - 1) / kTile;
     int64_t grid = (int64_t)m->sm_count * ctas_per_sm;
