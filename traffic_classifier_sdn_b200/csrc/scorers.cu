@@ -23,6 +23,7 @@
 // relative to its own terms (<= 1e-11 of the row's largest |jll| in the tests, labels unchanged).
 #include <cfloat>
 #include <cstdlib>
+#include <utility>
 
 #include "common.h"
 
@@ -422,8 +423,14 @@ static int launch_tiled_cfg(tcsdn_model *m, const T *x, int64_t n, int32_t *labe
     int64_t n_tiles = (n + kTile - 1) / kTile;
     int64_t grid = (int64_t)m->sm_count * ctas_per_sm;
     if (grid > n_tiles) grid = n_tiles;
-    // (Plain launches: with programmatic dependent launch, a correct griddepcontrol.wait has to precede the first load --
-    // the previous kernel may be the producer of X -- and early-launched CTAs of the next grid would sit on the SMs waiting.)
+    // Plain launches.  Programmatic dependent launch was measured and does not pay: in a CUDA graph of back-to-back 1M-row
+    // GaussianNB predicts the next scorer already starts when the previous one ends (torch.profiler: median end -> start gap
+    // -0.1 us, H100 80GB HBM3 at 700 W).  With the launch attribute, launch_dependents after the prologue and
+    // griddepcontrol.wait ahead of every global access (the previous kernel may be the producer of X), the next grid's
+    // CTAs were resident 20 us early and the step still took 15.0 us against 14.9 us (five alternated runs each).  Triggering
+    // once each CTA has issued its last load and prefetching the next grid's first tiles into L2 before its wait was slower
+    // still (15.3 us; 1 218 us against 1 173 us at 100M rows).  What is left of a 1M-row step is first-tile latency and the
+    // drain, not the launch; launch_tiled picks the shape that leaves the fewest CTAs idle in the drain.
     // fp32 pre-pass: GaussianNB, float32 rows, labels only (TCSDN_OPT_ENGINE = 1 routes to the generic fp64 kernel instead)
     unsigned long long *refined = (KIND == KIND_GNB && sizeof(T) == 4 && scores == nullptr) ? m->d_refined : nullptr;
     kern<<<(unsigned)grid, kThreads, smem, st>>>(m->sp, x, n, labels, scores, flag, refined, G);
@@ -436,14 +443,24 @@ static int launch_tiled(tcsdn_model *m, const T *x, int64_t n, int32_t *labels, 
                         cudaStream_t st, const GatherOut &G) {
     // CTA shape: GaussianNB wants the constants amortised over 4 rows (128 threads x 4), the HBM-bound max/min scorers want
     // more warps (256 x 2).
-    // Small batches: with 512-row tiles a 1M-row batch is 4.4 tiles per CTA -- the pipeline ramp (first tile) and the tail
-    // (some CTAs own one tile more) are a quarter of the step -- so below 16 tiles per CTA the 256-row shape (128 x 2) is used.
+    // Small batches (below 16 tiles per CTA): the pipeline ramp (first tile) and the tail are a large share of the step.  A CTA
+    // takes tiles round-robin, so in the last round only some CTAs have a tile and the others idle; that share depends on
+    // the batch size and the tile count, not only on the tile size.  The 256-row shape (128 x 2, one CTA per SM more) is used
+    // unless the default 512-row shape leaves fewer CTA-rounds idle: at 1M float32 rows on 132 SMs, 128 x 4 runs 1 954 tiles
+    // on 396 CTAs in 5 rounds (1.3 % idle), 128 x 2 runs 3 907 tiles on 528 CTAs in 8 rounds (7.5 % idle).
     // TCSDN_OPT_SCORER_SHAPE = 1 / 2 / 3 forces 128 x 4 / 256 x 2 / 128 x 2.
     const int per_sm = sizeof(T) == 4 ? 3 : 2;
     int shape = (int)m->opt_scorer_shape;
     if (shape == 0) {
         shape = KIND != KIND_GNB ? 2 : 1;
-        if ((n + 511) / 512 < (int64_t)16 * m->sm_count * per_sm) shape = 3;
+        auto idle = [&](int64_t tile_rows, int64_t ctas) {   // idle share of the CTA-rounds, as idle / total (cross-multiplied)
+            const int64_t tiles = (n + tile_rows - 1) / tile_rows, grid = tiles < ctas ? tiles : ctas;
+            const int64_t slots = (tiles + grid - 1) / grid * grid;
+            return std::make_pair(slots - tiles, slots);
+        };
+        const auto wide = idle(512, (int64_t)m->sm_count * per_sm), narrow = idle(256, (int64_t)m->sm_count * (per_sm + 1));
+        if ((n + 511) / 512 < (int64_t)16 * m->sm_count * per_sm && narrow.first * wide.second <= wide.first * narrow.second)
+            shape = 3;
     }
     if (shape == 2) return launch_tiled_cfg<T, D, R, KIND, 256, 2>(m, x, n, labels, scores, flag, st, per_sm, G);
     if (shape == 3) return launch_tiled_cfg<T, D, R, KIND, 128, 2>(m, x, n, labels, scores, flag, st, per_sm + 1, G);
