@@ -96,9 +96,21 @@ int tcsdn_gnb_create(const double *theta, const double *var, const double *class
 int tcsdn_kmeans_create(const double *centers, int32_t k, int32_t d, tcsdn_model_t **out);
 
 /* KNeighborsClassifier(weights='uniform', euclidean): _fit_X [n_train][d], _y [n_train] class index
- * in [0,n_classes).  sk:neighbors/_classification.py:245-312, sk:utils/_heap.pyx:6-88. */
+ * in [0,n_classes).  sk:neighbors/_classification.py:245-312, sk:utils/_heap.pyx:6-88.
+ * The same as tcsdn_knn_create_weighted(..., TCSDN_KNN_UNIFORM, out). */
 int tcsdn_knn_create(const double *fit_x, const int32_t *y, int64_t n_train, int32_t d,
                      int32_t n_classes, int32_t k, tcsdn_model_t **out);
+
+enum { TCSDN_KNN_UNIFORM = 0, TCSDN_KNN_DISTANCE = 1 }; /* tcsdn_knn_create_weighted() weights */
+
+/* KNeighborsClassifier(weights='uniform' | 'distance', euclidean): as tcsdn_knn_create, with the vote's weighting.
+ * TCSDN_KNN_DISTANCE (sk:neighbors/_base.py:74-114): the k neighbours, in ascending (distance, training index) order,
+ * weigh 1 / distance -- or, when any of them is at distance 0, 1 for those and 0 for the others; the label is the lowest
+ * class with the largest weight sum (numpy's pairwise row sum, sk:utils/extmath.py:791-862) and scores_out receives
+ * predict_proba (class sums in column order over their numpy row sum, sk:neighbors/_classification.py:398-410).  Any other
+ * weights value returns TCSDN_EINVAL.  tcsdn_knn_kneighbors does not depend on the weighting. */
+int tcsdn_knn_create_weighted(const double *fit_x, const int32_t *y, int64_t n_train, int32_t d,
+                              int32_t n_classes, int32_t k, int32_t weights, tcsdn_model_t **out);
 
 /* SVC(kernel='rbf'): support_vectors_ [n_sv][d] grouped by class, _dual_coef_ [n_classes-1][n_sv],
  * _intercept_ [n_classes*(n_classes-1)/2], _n_support [n_classes], _gamma.
@@ -120,7 +132,8 @@ void tcsdn_destroy(tcsdn_model_t *m);
 int tcsdn_model_kind(const tcsdn_model_t *m);
 int tcsdn_model_n_features(const tcsdn_model_t *m);
 /* columns of scores_out: linear n_rows (decision_function), gnb n_classes (joint log likelihood),
- * kmeans k (||c||^2 - 2 x.c), knn n_classes (neighbour votes / k), svc n_classes*(n_classes-1)/2
+ * kmeans k (||c||^2 - 2 x.c), knn n_classes (neighbour votes / k, or distance-weighted votes normalised),
+ * svc n_classes*(n_classes-1)/2
  * (libsvm's one-vs-one decision values), forest n_classes (predict_proba). */
 int tcsdn_model_score_cols(const tcsdn_model_t *m);
 int tcsdn_set_option(tcsdn_model_t *m, int32_t key, int64_t value);

@@ -16,6 +16,7 @@ OK, EINVAL, ECUDA, ENOMEM, ENONFINITE = 0, -1, -2, -3, -4
 OPT_ENGINE, OPT_CHUNK_ROWS, OPT_CHECK_FINITE = 1, 2, 3
 OPT_SCORER_SHAPE, OPT_FOREST_SHAPE, OPT_FOREST_SORT, OPT_KNN_FLUSH_TILES, OPT_KNN_PRUNE = 4, 5, 6, 7, 8
 FLOW_STATE = 19
+KNN_UNIFORM, KNN_DISTANCE = 0, 1
 COMM_ID_BYTES = 128
 
 _vp = C.c_void_p
@@ -34,6 +35,8 @@ SIGNATURES = {
     "tcsdn_gnb_create": (C.c_int, [_f64p, _f64p, _f64p, C.c_int32, C.c_int32, C.POINTER(_vp)]),
     "tcsdn_kmeans_create": (C.c_int, [_f64p, C.c_int32, C.c_int32, C.POINTER(_vp)]),
     "tcsdn_knn_create": (C.c_int, [_f64p, _i32p, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.POINTER(_vp)]),
+    "tcsdn_knn_create_weighted": (C.c_int, [_f64p, _i32p, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                            C.POINTER(_vp)]),
     "tcsdn_svc_create": (C.c_int, [_f64p, _f64p, _f64p, _i32p, C.c_int32, C.c_int32, C.c_int32, C.c_double,
                                    C.POINTER(_vp)]),
     "tcsdn_forest_create": (C.c_int, [_i64p, _i32p, _i32p, _i32p, _f64p, _f64p, C.c_int32, C.c_int32, C.c_int32,

@@ -281,8 +281,17 @@ int tcsdn_kmeans_create(const double *centers, int32_t k, int32_t d, tcsdn_model
 
 int tcsdn_knn_create(const double *fit_x, const int32_t *y, int64_t n_train, int32_t d, int32_t n_classes, int32_t k,
                      tcsdn_model_t **out) {
+    return tcsdn_knn_create_weighted(fit_x, y, n_train, d, n_classes, k, TCSDN_KNN_UNIFORM, out);
+}
+
+int tcsdn_knn_create_weighted(const double *fit_x, const int32_t *y, int64_t n_train, int32_t d, int32_t n_classes, int32_t k,
+                              int32_t weights, tcsdn_model_t **out) {
     if (!out) { set_error("out handle pointer is NULL"); return TCSDN_EINVAL; }
     *out = nullptr;
+    if (weights != TCSDN_KNN_UNIFORM && weights != TCSDN_KNN_DISTANCE) {
+        set_error("knn: weights must be TCSDN_KNN_UNIFORM or TCSDN_KNN_DISTANCE, got %d", weights);
+        return TCSDN_EINVAL;
+    }
     if (!fit_x || !y || n_train < 1 || n_classes < 1 || n_classes > 256) { set_error("knn: bad arguments"); return TCSDN_EINVAL; }
     if (k < 1 || k > 64 || k > n_train) { set_error("knn: need 1 <= k <= min(64, n_train), got k=%d n_train=%lld", k, (long long)n_train); return TCSDN_EINVAL; }
     if (n_train > (int64_t)INT32_MAX) { set_error("knn: n_train too large"); return TCSDN_EINVAL; }
@@ -291,7 +300,7 @@ int tcsdn_knn_create(const double *fit_x, const int32_t *y, int64_t n_train, int
         if (y[i] < 0 || y[i] >= n_classes) { set_error("knn: label index out of range"); return TCSDN_EINVAL; }
     tcsdn_model *m;
     TCSDN_TRY(model_base(&m, TCSDN_KIND_KNN, d, n_classes, n_classes));
-    m->n_train = n_train; m->k = k;
+    m->n_train = n_train; m->k = k; m->knn_weights = weights;
     int r = upload(&m->d_fit, fit_x, (size_t)n_train * d);
     if (r == TCSDN_OK) r = upload(&m->d_y, y, (size_t)n_train);
     if (r == TCSDN_OK) r = engine_create(m);

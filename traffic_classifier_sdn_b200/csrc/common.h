@@ -88,11 +88,10 @@ __device__ __forceinline__ void peer_flag_wait(const GatherOut &G, int which, un
     }
 }
 
-// KNeighbors.kneighbors: one query's m kept neighbours (squared distance, training index), slot i at values[i * ST], sorted
-// in place into ascending (distance, index) order and written as one row of ind (and of dist = sqrt, correctly rounded, when
-// dist is non-null).  m <= 64: an insertion sort is all it needs.
+// One query's m kept neighbours (squared distance, training index), slot i at values[i * ST], sorted in place into the
+// canonical ascending (distance, index) order.  m <= 64: an insertion sort is all it needs.
 template <int ST>
-__device__ __forceinline__ void knn_write_neighbors(double *values, int32_t *indices, int m, int64_t *ind, double *dist) {
+__device__ __forceinline__ void knn_sort_neighbors(double *values, int32_t *indices, int m) {
     for (int i = 1; i < m; ++i) {
         const double v = values[i * ST];
         const int32_t x = indices[i * ST];
@@ -104,9 +103,107 @@ __device__ __forceinline__ void knn_write_neighbors(double *values, int32_t *ind
         values[(j + 1) * ST] = v;
         indices[(j + 1) * ST] = x;
     }
+}
+
+// KNeighbors.kneighbors: the neighbours in canonical order, written as one row of ind (and of dist = sqrt, correctly rounded,
+// when dist is non-null)
+template <int ST>
+__device__ __forceinline__ void knn_write_neighbors(double *values, int32_t *indices, int m, int64_t *ind, double *dist) {
+    knn_sort_neighbors<ST>(values, indices, m);
     for (int i = 0; i < m; ++i) {
         ind[i] = indices[i * ST];
         if (dist) dist[i] = __dsqrt_rn(values[i * ST]);
+    }
+}
+
+// numpy's float64 row sum (np.sum(a, axis=1), pairwise_sum in numpy/_core/src/umath/loops_utils.h.src) of the n <= 128 terms
+// term(lo) .. term(lo + n - 1): sequential from 0.0 below 8 terms; else eight accumulators seeded with the first eight
+// terms, the following whole groups of 8 added column-wise, the accumulators combined as ((r0+r1)+(r2+r3))+((r4+r5)+(r6+r7)),
+// the remainder added sequentially.  No FMA contraction can change an association: every add is __dadd_rn.
+template <typename F>
+__device__ __forceinline__ double np_sum_block(const F &term, int lo, int n) {
+    if (n < 8) {
+        double res = 0.0;
+        for (int i = 0; i < n; ++i) res = __dadd_rn(res, term(lo + i));
+        return res;
+    }
+    double r[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) r[j] = term(lo + j);
+    int i = 8;
+    for (; i < n - (n % 8); i += 8) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) r[j] = __dadd_rn(r[j], term(lo + i + j));
+    }
+    double res = __dadd_rn(__dadd_rn(__dadd_rn(r[0], r[1]), __dadd_rn(r[2], r[3])), __dadd_rn(__dadd_rn(r[4], r[5]), __dadd_rn(r[6], r[7])));
+    for (; i < n; ++i) res = __dadd_rn(res, term(lo + i));
+    return res;
+}
+
+// the same for n <= 256 terms: above 128 numpy splits at n2 = n/2 - (n/2) % 8 and adds the two halves' sums, recursively
+// (two levels reach 256)
+template <typename F>
+__device__ __forceinline__ double np_sum(const F &term, int n) {
+    auto split = [](int len) { return len / 2 - (len / 2) % 8; };
+    const int nh = n > 128 ? 2 : 1, h0 = nh == 2 ? split(n) : n;
+    double res = 0.0;
+#pragma unroll 1
+    for (int h = 0; h < nh; ++h) {
+        const int lo = h == 0 ? 0 : h0, len = h == 0 ? h0 : n - h0;
+        const int np_ = len > 128 ? 2 : 1, p0 = np_ == 2 ? split(len) : len;
+        double half = 0.0;
+#pragma unroll 1
+        for (int p = 0; p < np_; ++p) {   // (first part) + (second part): the first part is not added to 0.0
+            const double v = np_sum_block(term, p == 0 ? lo : lo + p0, p == 0 ? p0 : len - p0);
+            half = p == 0 ? v : __dadd_rn(half, v);
+        }
+        res = h == 0 ? half : __dadd_rn(res, half);
+    }
+    return res;
+}
+
+// KNeighborsClassifier(weights='distance') for one query (sk:neighbors/_base.py:74-114, _classification.py:281-307,398-410,
+// sk:utils/extmath.py:791-862): values / indices hold the k kept neighbours as (squared distance, training index), slot i at
+// [i * ST]; y maps a training index to its class.  The slots are sorted into canonical (distance, index) order and then
+// overwritten with (weight, class):
+//   weight  w_i = 1 / sqrt(d_i), both correctly rounded; if any d_i == 0, w_i = 1 where d_i == 0 and 0 elsewhere
+//   label   per class c, W_c = numpy's row sum (np_sum_block) of the k columns of template_c = (w_i if y_i == c else 0.0);
+//           the lowest class with the largest W_c (weighted_mode: strict > in class order)
+//   proba   (non-null: C entries) P_c = 0.0 + the w_i of class c, sequentially in column order; P_c / (numpy's row sum of
+//           P_0 .. P_{C-1}).  The two sums associate differently, so the label may differ from argmax(proba) in the last
+//           bit exactly as sklearn's may.
+template <int ST>
+__device__ __forceinline__ void knn_weighted_vote(double *values, int32_t *indices, int k, int C, const int32_t *__restrict__ y,
+                                                  int32_t *label, double *proba) {
+    knn_sort_neighbors<ST>(values, indices, k);
+    const bool zero = values[0] == 0.0;   // sorted: a zero distance comes first
+    for (int i = 0; i < k; ++i) {
+        const double v = values[i * ST];
+        values[i * ST] = zero ? (v == 0.0 ? 1.0 : 0.0) : __ddiv_rn(1.0, __dsqrt_rn(v));
+        indices[i * ST] = y[indices[i * ST]];
+    }
+    if (proba)
+        for (int c = 0; c < C; ++c) proba[c] = 0.0;
+    double best = -1.0;
+    int arg = 0;
+    for (int i = 0; i < k; ++i) {   // each class present among the neighbours, at its first column
+        const int32_t c = indices[i * ST];
+        bool seen = false;
+        for (int j = 0; j < i; ++j) seen |= indices[j * ST] == c;
+        if (seen) continue;
+        const double W = np_sum_block([&](int t) { return indices[t * ST] == c ? values[t * ST] : 0.0; }, 0, k);
+        if (W > best || (W == best && c < arg)) { best = W; arg = c; }
+        if (proba) {
+            double p = 0.0;
+            for (int t = i; t < k; ++t)
+                if (indices[t * ST] == c) p = __dadd_rn(p, values[t * ST]);
+            proba[c] = p;
+        }
+    }
+    *label = arg;
+    if (proba) {
+        const double s = np_sum([&](int c) { return proba[c]; }, C);
+        for (int c = 0; c < C; ++c) proba[c] = __ddiv_rn(proba[c], s);
     }
 }
 
@@ -158,6 +255,7 @@ struct tcsdn_model {
     int32_t *d_y = nullptr;    // [n_train]
     int64_t n_train = 0;
     int k = 0;
+    int knn_weights = 0;       // TCSDN_KNN_UNIFORM or TCSDN_KNN_DISTANCE (predict only; kneighbors ignores it)
 
     // ---- svc
     double *d_sv = nullptr;      // [n_sv][d]

@@ -28,6 +28,8 @@
 // final k-th distance; if such a row and the kept rows at that distance do not all carry one class, the query goes to the
 // index-order fp64 kernel (knn.cu, marked mode) in the same call; otherwise every choice gives the same class counts.
 // kneighbors (NC1 bit 2) returns the SET, so there any row left out at the final k-th distance sends the query to that kernel.
+// The distance-weighted vote (NC1 bit 3, weights='distance') keeps the class rule: equally distant rows weigh the same, so
+// where every tied row carries one class, every choice gives the same (weight, class) columns in canonical order.
 // SVC uses acc directly, for LABELS only: e = -gamma log2(e) (acc + ||x' - c'_j||^2), K = ex2(e), C-1 fp32 FMAs per pair into
 // the running sums of the support vector's class, tile sums promoted to fp64.  To keep the fp32 accumulation error small
 // where K is not negligible, support vectors are re-ordered inside their class into spatially compact tiles and every tile
@@ -171,7 +173,7 @@ struct EngineArgs {
     const double *center;
     const double *ref;       // original fp64 reference rows (audit statistic)
     const double *refpad;    // the same rows at a 16-byte-aligned stride of dpad doubles (KNN exact re-evaluation)
-    const int32_t *y;        // KNN labels (original order; unused by the engine since the tiles are in kd order)
+    const int32_t *y;        // KNN labels (original order: the distance-weighted vote reads them by training index)
     const int32_t *ypos;     // KNN labels in tile order
     const int32_t *qperm;    // KNN: this call's query order (sorted by home tile) or nullptr = as given
     const int32_t *qkey;     // KNN: kd leaf per query (by original index)
@@ -750,7 +752,8 @@ engine_kernel(const __grid_constant__ EngineArgs A, const T *__restrict__ X, int
                 // memory.  Its root and the filter threshold stay in registers.
                 constexpr bool kHeapSmem = (NC1 & 1) != 0;      // KNN instantiations: NC1 bit 0 = heap in shared memory,
                 constexpr bool kAudit = (NC1 & 2) != 0;         //                     bit 1 = audit mode (error statistic),
-                constexpr bool kKnb = (NC1 & 4) != 0;           //                     bit 2 = kneighbors (rows of A.nb_ind / A.nb_dist)
+                constexpr bool kKnb = (NC1 & 4) != 0;           //                     bit 2 = kneighbors (rows of A.nb_ind / A.nb_dist),
+                constexpr bool kWd = (NC1 & 8) != 0;            //                     bit 3 = distance-weighted vote
                 constexpr int ST = kHeapSmem ? kKnnRows : 1;
                 double hv_local[kHeapSmem ? 1 : kEMaxK];
                 int32_t hi_local[kHeapSmem ? 1 : kEMaxK];
@@ -972,6 +975,10 @@ engine_kernel(const __grid_constant__ EngineArgs A, const T *__restrict__ X, int
                     } else if constexpr (kKnb) {
                         for (int i = 0; i < A.k; ++i) hi[i * ST] = A.pos_orig[hi[i * ST]];
                         knn_write_neighbors<ST>(hv, hi, A.k, A.nb_ind + row * A.k, A.nb_dist ? A.nb_dist + row * A.k : nullptr);
+                    } else if constexpr (kWd) {
+                        // equal distances are ordered by TRAINING index: map the tile positions before the sort
+                        for (int i = 0; i < A.k; ++i) hi[i * ST] = A.pos_orig[hi[i * ST]];
+                        knn_weighted_vote<ST>(hv, hi, A.k, A.C, A.y, labels + row, scores ? scores + row * A.C : nullptr);
                     } else {
                         int best = 0, arg = 0;
                         for (int c = 0; c < A.C; ++c) {
@@ -1726,7 +1733,9 @@ static int launch_engine_t(tcsdn_model *m, const T *x, int64_t n, int32_t *label
         kern<<<grid, SVCF ? kESvcThreads : kEKnnThreads, smem, st>>>(A, x, labels, scores, E->d_counters);        \
     }
     if (!svc) {
-        const int variant = (heap_smem ? 1 : 0) | (A.maxratio ? 2 : 0) | (nb_ind ? 4 : 0);
+        // the distance-weighted vote (bit 3) belongs to predict on weights='distance' handles; kneighbors has no vote
+        const bool wd = !nb_ind && m->knn_weights == TCSDN_KNN_DISTANCE;
+        const int variant = (heap_smem ? 1 : 0) | (A.maxratio ? 2 : 0) | (nb_ind ? 4 : 0) | (wd ? 8 : 0);
         switch (variant) {
             case 0: TCSDN_LAUNCH(false, 0) break;
             case 1: TCSDN_LAUNCH(false, 1) break;
@@ -1734,7 +1743,9 @@ static int launch_engine_t(tcsdn_model *m, const T *x, int64_t n, int32_t *label
             case 3: TCSDN_LAUNCH(false, 3) break;
             case 4: TCSDN_LAUNCH(false, 4) break;
             case 5: TCSDN_LAUNCH(false, 5) break;
-            default: set_error("knn engine: kneighbors has no audit mode"); return TCSDN_EINVAL;
+            case 8: TCSDN_LAUNCH(false, 8) break;
+            case 9: TCSDN_LAUNCH(false, 9) break;
+            default: set_error("knn engine: kneighbors and distance weights have no audit mode"); return TCSDN_EINVAL;
         }
     }
     else switch (E->nc1) {

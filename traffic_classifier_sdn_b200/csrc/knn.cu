@@ -11,7 +11,8 @@
 // engine's exact re-evaluation rule, and as the engine's cross-check in the tests.  One thread owns one
 // query and scans the training rows in index order out of a shared-memory tile (all lanes read the same
 // training row: broadcast), so the heap sees exactly sklearn's push sequence.  Both kernels have a kneighbors mode (template
-// flag KNB): the same heap, then the kept rows in ascending (distance, index) order instead of the vote.
+// flag KNB): the same heap, then the kept rows in ascending (distance, index) order instead of the vote; and a distance-weighted
+// vote (template flag WD, weights='distance'): the same heap, then knn_weighted_vote (common.h) instead of the count.
 #include <cfloat>
 
 #include "common.h"
@@ -47,7 +48,8 @@ __device__ __forceinline__ void heap_push_dev(double *values, int32_t *indices, 
 
 // KNB (kneighbors): instead of the vote, the k kept rows in ascending (distance, index) order go to nb_ind / nb_dist
 // [n][k] (nb_dist nullable); labels and proba are unused.  The predict instantiation ignores the two trailing arguments.
-template <typename T, bool KNB = false>
+// WD (weights='distance'): label and proba from the distance-weighted vote.
+template <typename T, bool KNB = false, bool WD = false>
 __global__ void __launch_bounds__(kKnnThreads) knn_exact_kernel(const T *__restrict__ X, int64_t n, int d,
                                                                 const double *__restrict__ fit,
                                                                 const int32_t *__restrict__ y, int64_t n_train,
@@ -91,6 +93,8 @@ __global__ void __launch_bounds__(kKnnThreads) knn_exact_kernel(const T *__restr
         }
         if constexpr (KNB) {
             if (live) knn_write_neighbors<1>(hv, hi, k, nb_ind + q * k, nb_dist ? nb_dist + q * k : nullptr);
+        } else if constexpr (WD) {
+            if (live) knn_weighted_vote<1>(hv, hi, k, C, y, labels + q, proba ? proba + q * C : nullptr);
         } else if (live) {
             int best = 0, arg = 0;
             for (int c = 0; c < C; ++c) {
@@ -116,13 +120,15 @@ static int launch_exact(tcsdn_model *m, const void *x, int64_t n, int dtype, int
     if (blocks > cap) blocks = cap;
     m->stats[0] += 1;
     m->stats[2] += n;
+    // the distance-weighted vote is a predict mode of weights='distance' handles; kneighbors has no vote
+    const bool wd = !KNB && m->knn_weights == TCSDN_KNN_DISTANCE;
     if (dtype == TCSDN_F32) {
-        auto kern = knn_exact_kernel<float, KNB>;
+        auto kern = wd ? knn_exact_kernel<float, KNB, !KNB> : knn_exact_kernel<float, KNB, false>;
         TCSDN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kern<<<(unsigned)blocks, kKnnThreads, smem, st>>>(static_cast<const float *>(x), n, m->d, m->d_fit, m->d_y,
                                                           m->n_train, k, m->n_classes, labels, scores, flag, nb_ind, nb_dist);
     } else {
-        auto kern = knn_exact_kernel<double, KNB>;
+        auto kern = wd ? knn_exact_kernel<double, KNB, !KNB> : knn_exact_kernel<double, KNB, false>;
         TCSDN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kern<<<(unsigned)blocks, kKnnThreads, smem, st>>>(static_cast<const double *>(x), n, m->d, m->d_fit, m->d_y,
                                                           m->n_train, k, m->n_classes, labels, scores, flag, nb_ind, nb_dist);
@@ -147,8 +153,9 @@ int launch_knn_exact_kneighbors(tcsdn_model *m, const void *x, int64_t n, int dt
 // in step -- the sequential heap's result at 1/32 of its latency.  The number of rows is only known on the device.
 constexpr int kTieMaxD = 12;   // the engine's feature limit
 
-// KNB (kneighbors): lane 0 writes the k kept rows in ascending (distance, index) order to nb_ind / nb_dist instead of the vote
-template <typename T, bool KNB = false>
+// KNB (kneighbors): lane 0 writes the k kept rows in ascending (distance, index) order to nb_ind / nb_dist instead of the vote;
+// WD (weights='distance'): lane 0 casts the distance-weighted vote
+template <typename T, bool KNB = false, bool WD = false>
 __global__ void __launch_bounds__(256) knn_tie_kernel(const T *__restrict__ X, int d, const double *__restrict__ fit,
                                                       const int32_t *__restrict__ y, int64_t n_train, int k, int C,
                                                       int32_t *__restrict__ labels, double *__restrict__ proba,
@@ -200,6 +207,8 @@ __global__ void __launch_bounds__(256) knn_tie_kernel(const T *__restrict__ X, i
         }
         if constexpr (KNB) {
             if (lane == 0) knn_write_neighbors<1>(hv, hi, k, nb_ind + q * k, nb_dist ? nb_dist + q * k : nullptr);
+        } else if constexpr (WD) {
+            if (lane == 0) knn_weighted_vote<1>(hv, hi, k, C, y, labels + q, proba ? proba + q * C : nullptr);
         } else if (lane == 0) {
             int best = 0, arg = 0;
             for (int c = 0; c < C; ++c) {
@@ -223,12 +232,16 @@ static int launch_marked(tcsdn_model *m, const void *x, int64_t n, int dtype, in
     const int64_t cap = (int64_t)m->sm_count * 4;
     if (blocks > cap) blocks = cap;
     m->stats[0] += 1;
-    if (dtype == TCSDN_F32)
-        knn_tie_kernel<float, KNB><<<(unsigned)blocks, 256, 0, st>>>(static_cast<const float *>(x), m->d, m->d_fit, m->d_y, m->n_train,
-                                                                     k, m->n_classes, labels, scores, list, count, total, nb_ind, nb_dist);
-    else
-        knn_tie_kernel<double, KNB><<<(unsigned)blocks, 256, 0, st>>>(static_cast<const double *>(x), m->d, m->d_fit, m->d_y, m->n_train,
-                                                                      k, m->n_classes, labels, scores, list, count, total, nb_ind, nb_dist);
+    const bool wd = !KNB && m->knn_weights == TCSDN_KNN_DISTANCE;
+    if (dtype == TCSDN_F32) {
+        auto kern = wd ? knn_tie_kernel<float, KNB, !KNB> : knn_tie_kernel<float, KNB, false>;
+        kern<<<(unsigned)blocks, 256, 0, st>>>(static_cast<const float *>(x), m->d, m->d_fit, m->d_y, m->n_train, k, m->n_classes,
+                                               labels, scores, list, count, total, nb_ind, nb_dist);
+    } else {
+        auto kern = wd ? knn_tie_kernel<double, KNB, !KNB> : knn_tie_kernel<double, KNB, false>;
+        kern<<<(unsigned)blocks, 256, 0, st>>>(static_cast<const double *>(x), m->d, m->d_fit, m->d_y, m->n_train, k, m->n_classes,
+                                               labels, scores, list, count, total, nb_ind, nb_dist);
+    }
     TCSDN_CUDA(cudaGetLastError());
     return TCSDN_OK;
 }

@@ -426,7 +426,8 @@ class KMeans(_Base):
 
 
 class KNeighborsClassifier(_Base):
-    """sk:neighbors/_classification.py:245-312 -- k nearest (euclidean, heap order), uniform vote."""
+    """sk:neighbors/_classification.py:245-312 -- k nearest (euclidean, heap order), uniform or distance-weighted vote
+    (``weights='uniform'`` / ``'distance'``; sk:neighbors/_base.py:74-114)."""
     _kind = "knn"
 
     def __init__(self, n_neighbors=5, **params):
@@ -439,9 +440,21 @@ class KNeighborsClassifier(_Base):
     def _create(self, lib, spec, h):
         fx = np.ascontiguousarray(spec["fit_X"], np.float64)
         y = np.ascontiguousarray(spec["y"], np.int32)
+        weights = modelio.knn_weights(spec.get("weights", "uniform"))
         self.n_samples_fit_ = fx.shape[0]
-        _lib.check(lib.tcsdn_knn_create(_p(fx, _lib._f64p), _p(y, _lib._i32p), fx.shape[0], fx.shape[1],
-                                        len(spec["classes"]), int(spec["k"]), C.byref(h)))
+        self.weights = weights
+        _lib.check(lib.tcsdn_knn_create_weighted(_p(fx, _lib._f64p), _p(y, _lib._i32p), fx.shape[0], fx.shape[1],
+                                                 len(spec["classes"]), int(spec["k"]),
+                                                 _lib.KNN_DISTANCE if weights == "distance" else _lib.KNN_UNIFORM, C.byref(h)))
+
+    def set_params(self, **params):
+        """sklearn applies ``weights`` at predict time, so on a fitted model a new weighting re-creates the handle from the
+        fitted spec (the handle's options, set_option, start from their defaults again)."""
+        if "weights" in params and self._spec is not None:
+            w = modelio.knn_weights(params["weights"])
+            if w != modelio.knn_weights(self._spec.get("weights", "uniform")):
+                self._adopt(dict(self._spec, weights=w))
+        return super().set_params(**params)
 
     def predict_proba(self, X):
         return self._scores(X)
@@ -605,6 +618,7 @@ def from_spec(spec):
         est._params["n_clusters"] = int(np.asarray(spec["centers"]).shape[0])
     if spec["kind"] == "knn":
         est._params["n_neighbors"] = int(spec["k"])
+        est._params["weights"] = modelio.knn_weights(spec.get("weights", "uniform"))
     return est._adopt(spec)
 
 

@@ -18,7 +18,8 @@ linear     coef [R,d] f64, intercept [R] f64, classes  (R == 1 means binary), ov
            one-vs-rest probabilities)
 gnb        theta [C,d], var [C,d], class_prior [C], classes
 kmeans     centers [k,d]
-knn        fit_X [n_t,d] f64, y [n_t] int32 (class index), k, classes
+knn        fit_X [n_t,d] f64, y [n_t] int32 (class index), k, classes, weights ("uniform" or
+           "distance"; a spec without the key is uniform)
 svc        sv [nSV,d], dual_coef [C-1,nSV], intercept [P], n_support [C] int32,
            gamma, classes, decision_function_shape, break_ties
 forest     tree_offsets [T+1] int64, left/right/feature int32 [N], threshold f64 [N],
@@ -34,7 +35,7 @@ from typing import Any, Dict
 import numpy as np
 
 __all__ = ["load_reference_pickle", "spec_from_estimator", "spec_from_pickle_bytes",
-           "MODEL_FILES", "SpecError"]
+           "knn_weights", "MODEL_FILES", "SpecError"]
 
 # argv word -> pickle file, as dispatched at reference traffic_classifier.py:229-240
 MODEL_FILES = {
@@ -144,6 +145,18 @@ def _tree_arrays(tree):
             np.asarray(feature, np.int32), _f64(threshold), np.ascontiguousarray(value))
 
 
+def knn_weights(w) -> str:
+    """KNeighborsClassifier's ``weights`` as a spec value: "uniform" (also for None, sklearn's older spelling) or
+    "distance".  A callable cannot become a kernel and is refused."""
+    if w is None or (isinstance(w, str) and w == "uniform"):
+        return "uniform"
+    if isinstance(w, str) and w == "distance":
+        return "distance"
+    if callable(w):
+        raise SpecError("callable weights are not implemented (weights must be 'uniform' or 'distance')")
+    raise SpecError(f"weights must be 'uniform' or 'distance', got {w!r}")
+
+
 def _spec_from_attrs(name: str, o) -> Dict[str, Any]:
     if name == "LogisticRegression":
         coef = _f64(o.coef_)
@@ -165,8 +178,7 @@ def _spec_from_attrs(name: str, o) -> Dict[str, Any]:
         return dict(kind="kmeans", centers=c, classes=np.arange(c.shape[0], dtype=np.int32),
                     n_features=c.shape[1])
     if name == "KNeighborsClassifier":
-        if getattr(o, "weights", "uniform") != "uniform":
-            raise SpecError("only weights='uniform' is implemented")
+        weights = knn_weights(getattr(o, "weights", "uniform"))
         metric = getattr(o, "effective_metric_", getattr(o, "metric", "minkowski"))
         p = getattr(o, "p", 2)
         if not (metric in ("euclidean", "l2") or (metric == "minkowski" and p == 2)):
@@ -176,7 +188,7 @@ def _spec_from_attrs(name: str, o) -> Dict[str, Any]:
         if y.ndim != 1:
             raise SpecError("multi-output KNN is not supported")
         return dict(kind="knn", fit_X=fx, y=np.ascontiguousarray(y, dtype=np.int32),
-                    k=int(o.n_neighbors), classes=_classes(o), n_features=fx.shape[1])
+                    k=int(o.n_neighbors), classes=_classes(o), n_features=fx.shape[1], weights=weights)
     if name == "SVC":
         if o.kernel != "rbf":
             raise SpecError("only kernel='rbf' is implemented")
