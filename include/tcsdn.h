@@ -181,13 +181,19 @@ int tcsdn_svc_ovr_from_ovo(const double *dec, int64_t n, int32_t n_classes, int3
  * (the other four estimators keep importing fitted parameters from scikit-learn).  X [n][d] float32/float64 and
  * y / labels_out live where `loc` says; the small outputs (theta, var, ..., centers_out) are HOST arrays.
  * Sums are fp64 and deterministic but not in numpy's order: results agree with scikit-learn to ~1e-13 relative.
+ * float32 rows are fitted in fp64 (scikit-learn's fit of the widened rows).  d <= 255.
  *
  * tcsdn_gnb_fit     GaussianNB.fit (sk:naive_bayes.py:385-476): y [n] class index in [0, n_classes);
  *                   theta/var [n_classes][d] (var includes epsilon = var_smoothing * max_j Var(X_j)),
  *                   class_prior [n_classes], class_count (nullable) [n_classes], epsilon (nullable).
  * tcsdn_kmeans_fit  KMeans(init=init_centers, n_init=1, algorithm="lloyd").fit (sk:cluster/_kmeans.py:620-760):
  *                   E-step fused with the M-step's sums per iteration; stops on unchanged labels or on
- *                   sum(center_shift^2) <= mean(Var(X_j)) * tol.  k <= 33.  labels_out (nullable) [n]. */
+ *                   sum(center_shift^2) <= mean(Var(X_j)) * tol.  k <= 33.  labels_out (nullable) [n], complete
+ *                   when the call returns.  An empty cluster is relocated as sklearn's _relocate_empty_clusters_dense
+ *                   does: to the row farthest from its centre, which leaves its own cluster (with three or more empty
+ *                   clusters in one iteration the far rows go in decreasing distance, lower row first on ties, where
+ *                   sklearn's order is undefined); a cluster still empty takes sklearn's _average_centers value
+ *                   (DESIGN §2, fit contract). */
 int tcsdn_gnb_fit(const void *x, const int32_t *y, int64_t n, int32_t d, int32_t n_classes, int32_t x_dtype,
                   int32_t loc, double var_smoothing, double *theta, double *var, double *class_prior,
                   double *class_count, double *epsilon, void *cuda_stream);

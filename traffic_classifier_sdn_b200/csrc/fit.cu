@@ -15,8 +15,10 @@
 // owns (row lane, column) and adds its rows in order, a block reduces its lanes in order, a final kernel adds the
 // blocks in order.  The summation order differs from numpy's, so fitted parameters agree with scikit-learn to ~1e-13
 // relative, not bit for bit (tests/test_fit_gpu.py states the tolerance).
+#include <algorithm>
 #include <cfloat>
 #include <cmath>
+#include <numeric>
 #include <vector>
 
 #include "common.h"
@@ -112,16 +114,32 @@ __global__ void moments_final_kernel(const double *partial, int blocks, int cell
     out[t] = s;
 }
 
+// KMeans empty-cluster relocation (sk:cluster/_k_means_common.pyx:186): dist[r] = ||x_r - center[label[r]]||^2 in fp64,
+// against the centres the E-step used.  Only launched on iterations that leave a cluster empty.
+template <typename T>
+__global__ void label_dist_kernel(const T *x, const int32_t *labels, const double *center, int64_t n, int d,
+                                  double *dist) {
+    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n) return;
+    const double *c = center + (size_t)labels[r] * d;
+    double s = 0.0;
+    for (int q = 0; q < d; ++q) {
+        const double dv = static_cast<double>(x[r * d + q]) - c[q];
+        s += dv * dv;
+    }
+    dist[r] = s;
+}
+
 struct FitScratch {
     void *d_x = nullptr; bool own_x = false;
     int32_t *d_y = nullptr; bool own_y = false;
-    double *d_center = nullptr, *d_partial = nullptr, *d_out = nullptr;
+    double *d_center = nullptr, *d_partial = nullptr, *d_out = nullptr, *d_dist = nullptr;
     int32_t *d_flag = nullptr, *d_labels = nullptr;
     int blocks = 0;
     ~FitScratch() {
         if (own_x) cudaFree(d_x);
         if (own_y) cudaFree(d_y);
-        cudaFree(d_center); cudaFree(d_partial); cudaFree(d_out); cudaFree(d_flag); cudaFree(d_labels);
+        cudaFree(d_center); cudaFree(d_partial); cudaFree(d_out); cudaFree(d_dist); cudaFree(d_flag); cudaFree(d_labels);
     }
 };
 
@@ -178,6 +196,55 @@ static int fit_pass(FitScratch &S, int64_t n, int d, int dtype, int G, int all_g
     out.resize((size_t)cells);
     TCSDN_CUDA(cudaMemcpyAsync(out.data(), S.d_out, (size_t)cells * 8, cudaMemcpyDeviceToHost, st));
     TCSDN_CUDA(cudaStreamSynchronize(st));
+    return TCSDN_OK;
+}
+
+// sk:cluster/_k_means_common.pyx:167-211 (_relocate_empty_clusters_dense) applied to the fused pass's sums [k][d+1]
+// (column d: the count).  S.d_center holds the centres the E-step used and S.d_labels its labels (`labels` on the host).
+// Every empty cluster, in index order, takes the next row in decreasing distance to its own centre (equal distances:
+// lower row first): the row leaves its cluster's sum and count and becomes the empty cluster's sum, count 1.  sklearn
+// takes the rows in numpy's argpartition order, which is the same for one or two empty clusters and undefined from
+// three on.  If every row sits exactly on its centre nothing moves, as in sklearn.
+static int relocate_empty(FitScratch &S, int64_t n, int d, int dtype, int k, const std::vector<int32_t> &labels,
+                          std::vector<double> &sums, cudaStream_t st) {
+    const int dp = d + 1;
+    std::vector<int> empty;
+    for (int c = 0; c < k; ++c)
+        if (sums[(size_t)c * dp + d] == 0.0) empty.push_back(c);
+    if (empty.empty()) return TCSDN_OK;
+    if (!S.d_dist) TCSDN_CUDA(cudaMalloc((void **)&S.d_dist, (size_t)n * 8));
+    const unsigned grid = (unsigned)((n + 255) / 256);
+    if (dtype == TCSDN_F32)
+        label_dist_kernel<float><<<grid, 256, 0, st>>>(static_cast<const float *>(S.d_x), S.d_labels, S.d_center, n, d, S.d_dist);
+    else
+        label_dist_kernel<double><<<grid, 256, 0, st>>>(static_cast<const double *>(S.d_x), S.d_labels, S.d_center, n, d, S.d_dist);
+    TCSDN_CUDA(cudaGetLastError());
+    std::vector<double> dist((size_t)n);
+    TCSDN_CUDA(cudaMemcpyAsync(dist.data(), S.d_dist, (size_t)n * 8, cudaMemcpyDeviceToHost, st));
+    TCSDN_CUDA(cudaStreamSynchronize(st));
+    const size_t m = empty.size();   // <= k <= n
+    std::vector<int64_t> far((size_t)n);
+    std::iota(far.begin(), far.end(), (int64_t)0);
+    std::partial_sort(far.begin(), far.begin() + m, far.end(), [&](int64_t a, int64_t b) {
+        return dist[a] > dist[b] || (dist[a] == dist[b] && a < b);
+    });
+    if (dist[far[0]] == 0.0) return TCSDN_OK;
+    const size_t es = dtype == TCSDN_F32 ? 4 : 8;
+    std::vector<unsigned char> raw((size_t)d * es);
+    for (size_t e = 0; e < m; ++e) {
+        const int64_t r = far[e];
+        const int to = empty[e], from = labels[(size_t)r];
+        TCSDN_CUDA(cudaMemcpy(raw.data(), static_cast<const unsigned char *>(S.d_x) + (size_t)r * d * es, (size_t)d * es,
+                              cudaMemcpyDeviceToHost));
+        for (int j = 0; j < d; ++j) {
+            const double v = dtype == TCSDN_F32 ? (double)reinterpret_cast<const float *>(raw.data())[j]
+                                                : reinterpret_cast<const double *>(raw.data())[j];
+            sums[(size_t)from * dp + j] -= v;
+            sums[(size_t)to * dp + j] = v;
+        }
+        sums[(size_t)from * dp + d] -= 1.0;
+        sums[(size_t)to * dp + d] = 1.0;
+    }
     return TCSDN_OK;
 }
 
@@ -268,18 +335,28 @@ int tcsdn_kmeans_fit(const void *x, int64_t n, int32_t d, int32_t k, int32_t x_d
     for (it = 0; it < max_iter; ++it) {
         // E-step (labels against `centers`) fused with the M-step's sums
         TCSDN_TRY(fit_pass(S, n, d, x_dtype, k, -1, 1, centers.data(), 0, S.d_labels, sums, st));
+        TCSDN_CUDA(cudaMemcpy(labels.data(), S.d_labels, (size_t)n * 4, cudaMemcpyDeviceToHost));
+        TCSDN_TRY(relocate_empty(S, n, d, x_dtype, k, labels, sums, st));
+        // a cluster still empty after relocation (no row off its centre, or a donor that gave its only row) takes what
+        // sk:cluster/_k_means_common.pyx:274-295 (_average_centers) gives it: the entry of the largest cluster (first
+        // maximum) as that loop has left it -- averaged if it comes earlier, else still its sum, which in sklearn's
+        // mean-centred rows is sum(x - mean), i.e. sum(x) - (count - 1) * mean here
+        int big = 0;
+        for (int c = 1; c < k; ++c)
+            if (sums[(size_t)c * dp + d] > sums[(size_t)big * dp + d]) big = c;
+        const double big_cnt = sums[(size_t)big * dp + d];
         double shift = 0.0;
         for (int c = 0; c < k; ++c) {
             const double cnt = sums[(size_t)c * dp + d];
             for (int j = 0; j < d; ++j) {
-                // an empty cluster keeps its centre (sklearn relocates it to the farthest point; with the inits the
-                // notebooks use this does not occur, and the caller is told through n_iter/inertia either way)
-                next[(size_t)c * d + j] = cnt > 0.0 ? sums[(size_t)c * dp + j] / cnt : centers[(size_t)c * d + j];
-                const double dv = next[(size_t)c * d + j] - centers[(size_t)c * d + j];
+                double &v = next[(size_t)c * d + j];
+                if (cnt > 0.0) v = sums[(size_t)c * dp + j] / cnt;
+                else if (big < c) v = next[(size_t)big * d + j];
+                else v = sums[(size_t)big * dp + j] - (big_cnt - 1.0) * mean[j];
+                const double dv = v - centers[(size_t)c * d + j];
                 shift += dv * dv;
             }
         }
-        TCSDN_CUDA(cudaMemcpy(labels.data(), S.d_labels, (size_t)n * 4, cudaMemcpyDeviceToHost));
         centers.swap(next);
         if (labels == labels_old) { strict = true; ++it; break; }
         if (shift <= tol_abs) { ++it; break; }
@@ -299,8 +376,12 @@ int tcsdn_kmeans_fit(const void *x, int64_t n, int32_t d, int32_t k, int32_t x_d
         for (int j = 0; j < d; ++j) inertia += sq[(size_t)c * dp + j];
     memcpy(centers_out, centers.data(), (size_t)k * d * 8);
     if (labels_out) {
-        if (loc == TCSDN_DEVICE) TCSDN_CUDA(cudaMemcpy(labels_out, S.d_labels, (size_t)n * 4, cudaMemcpyDeviceToDevice));
-        else memcpy(labels_out, labels.data(), (size_t)n * 4);
+        if (loc == TCSDN_DEVICE) {   // complete when the call returns, like the host outputs
+            TCSDN_CUDA(cudaMemcpyAsync(labels_out, S.d_labels, (size_t)n * 4, cudaMemcpyDeviceToDevice, st));
+            TCSDN_CUDA(cudaStreamSynchronize(st));
+        } else {
+            memcpy(labels_out, labels.data(), (size_t)n * 4);
+        }
     }
     if (inertia_out) *inertia_out = inertia;
     if (n_iter_out) *n_iter_out = it;

@@ -327,6 +327,10 @@ class GaussianNB(_Base):
         ptr, n, d, dt, loc, keep = self._fit_rows(X)
         if len(yi) != n:
             raise ValueError(f"Found input variables with inconsistent numbers of samples: [{n}, {len(yi)}]")
+        if len(classes) > 32 or d > 255:   # the fit kernel's per-block accumulators: classes + 1 <= 33, d + 1 <= 256
+            if strict:
+                raise ValueError(f"the GPU fit supports at most 32 classes and 255 features (got {len(classes)} and {d})")
+            return False
         yi = np.ascontiguousarray(yi, np.int32)
         ydev = None
         if loc == _lib.DEVICE:
@@ -392,6 +396,10 @@ class KMeans(_Base):
                                  "n_clusters <= 33")
             return False
         ptr, n, d, dt, loc, keep = self._fit_rows(X)
+        if d > 255:
+            if strict:
+                raise ValueError(f"the GPU fit supports at most 255 features (got {d})")
+            return False
         if isinstance(init, np.ndarray):
             c0 = np.ascontiguousarray(init, np.float64)
             if c0.shape != (k, d):
@@ -407,18 +415,19 @@ class KMeans(_Base):
             c0 = np.ascontiguousarray(c0 + mean, np.float64)
         ctr = np.empty((k, d))
         inertia, n_iter = C.c_double(0.0), C.c_int32(0)
-        labels = None
-        lptr = None
         if loc == _lib.HOST:
             labels = np.empty(n, np.int32)
             lptr = _p(labels, C.c_void_p)
+        else:
+            import torch
+            labels = torch.empty(n, dtype=torch.int32, device=keep.device)
+            lptr = C.c_void_p(labels.data_ptr())
         _lib.check(_lib.load().tcsdn_kmeans_fit(ptr, n, d, k, dt, loc, _p(c0, _lib._f64p), int(p.get("max_iter", 300)),
                                                 float(p.get("tol", 1e-4)), _p(ctr, _lib._f64p), lptr, C.byref(inertia),
                                                 C.byref(n_iter), None))
         self._adopt(dict(kind="kmeans", centers=ctr, classes=np.arange(k, dtype=np.int32), n_features=d))
         self.inertia_, self.n_iter_ = float(inertia.value), int(n_iter.value)
-        if labels is not None:
-            self.labels_ = labels
+        self.labels_ = labels if loc == _lib.HOST else labels.cpu().numpy()
         return True
 
     def fit_predict(self, X, y=None):
