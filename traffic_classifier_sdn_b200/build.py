@@ -31,14 +31,12 @@ def needs_build():
     return any(os.path.getmtime(p) > t for p in deps)
 
 
-def build(force=False, verbose=False, extra_flags=(), out=None):
-    """Compile every .cu for sm_90a and link libtcsdn.so.  Returns the library path.
-    `extra_flags` / `out`: experiment builds (e.g. -DTCSDN_EXP_NO_EX2) into another file, tools/ only."""
-    lib_out = out or LIB
-    if not force and not out and not needs_build():
+def build(force=False, verbose=False):
+    """Compile every .cu for sm_90a and link libtcsdn.so.  Returns the library path."""
+    if not force and not needs_build():
         return LIB
     nvcc = _nvcc()
-    objdir = os.path.join(HERE, "build" if not out else "build_" + os.path.basename(out))
+    objdir = os.path.join(HERE, "build")
     os.makedirs(objdir, exist_ok=True)
     env = dict(os.environ)
     env.pop("CC", None)
@@ -47,7 +45,7 @@ def build(force=False, verbose=False, extra_flags=(), out=None):
     for src in SOURCES:
         for objname, vflags in VARIANTS.get(src, [(src.replace(".cu", ".o"), [])]):
             obj = os.path.join(objdir, objname)
-            cmd = [nvcc, "-ccbin", "/usr/bin/g++"] + NVCC_FLAGS + list(extra_flags) + vflags + ["-c", os.path.join(CSRC, src), "-o", obj]
+            cmd = [nvcc, "-ccbin", "/usr/bin/g++"] + NVCC_FLAGS + vflags + ["-c", os.path.join(CSRC, src), "-o", obj]
             procs.append((f"{src} {' '.join(vflags)}".strip(), obj,
                           subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, env=env, text=True)))
     objs, log = [], []
@@ -60,11 +58,11 @@ def build(force=False, verbose=False, extra_flags=(), out=None):
         objs.append(obj)
     with open(os.path.join(objdir, "ptxas.log"), "w") as fh:
         fh.write("\n".join(log))
-    cmd = [nvcc, "-ccbin", "/usr/bin/g++", "-shared"] + NVCC_FLAGS[:2] + ["-o", lib_out] + objs + ["-lcuda", "-ldl"]
+    cmd = [nvcc, "-ccbin", "/usr/bin/g++", "-shared"] + NVCC_FLAGS[:2] + ["-o", LIB] + objs + ["-lcuda", "-ldl"]
     subprocess.check_call(cmd, env=env)
     if verbose:
         print("\n".join(log))
-    return lib_out
+    return LIB
 
 
 if __name__ == "__main__":

@@ -123,13 +123,13 @@ static int run_device(tcsdn_model *m, const void *x, int64_t n, int dtype, int32
         case TCSDN_KIND_KMEANS: return launch_scorer(m, x, n, dtype, labels, scores, flag, st);
         case TCSDN_KIND_FOREST: return launch_forest(m, x, n, dtype, labels, scores, flag, st);
         case TCSDN_KIND_KNN:
-            if (m->opt_engine != 1 && engine_usable(m, n, scores != nullptr)) return launch_engine(m, x, n, dtype, labels, scores, flag, st);
+            if (m->opt_engine != 1 && engine_usable(m, n, scores != nullptr)) return launch_knn_engine(m, x, n, dtype, labels, scores, flag, st);
             if (m->opt_engine >= 2) { set_error("tensor-core engine forced but not usable for this model/batch"); return TCSDN_EINVAL; }
             return launch_knn_exact(m, x, n, dtype, labels, scores, flag, st);
         case TCSDN_KIND_SVC:
             // decision values are always the fp64 kernel's (the engine certifies LABELS; its fp32 sums cannot meet a
             // 1e-5 absolute bound on decision values, see dist_engine.cu)
-            if (m->opt_engine != 1 && engine_usable(m, n, scores != nullptr)) return launch_engine(m, x, n, dtype, labels, scores, flag, st);
+            if (m->opt_engine != 1 && engine_usable(m, n, scores != nullptr)) return launch_svc_engine(m, x, n, dtype, labels, scores, flag, st);
             if (m->opt_engine >= 2 && !scores) { set_error("tensor-core engine forced but not usable for this model/batch"); return TCSDN_EINVAL; }
             return launch_svc_exact(m, x, n, dtype, labels, scores, flag, st);
     }
@@ -141,7 +141,7 @@ static int run_device(tcsdn_model *m, const void *x, int64_t n, int dtype, int32
 static int run_kneighbors(tcsdn_model *m, const void *x, int64_t n, int dtype, int nn, int64_t *ind, double *dist,
                           int32_t *flag, cudaStream_t st) {
     if (!m->opt_check_finite) flag = nullptr;
-    if (m->opt_engine != 1 && engine_kneighbors_usable(m, n, nn)) return launch_engine_kneighbors(m, x, n, dtype, nn, ind, dist, flag, st);
+    if (m->opt_engine != 1 && engine_kneighbors_usable(m, n, nn)) return launch_knn_engine_kneighbors(m, x, n, dtype, nn, ind, dist, flag, st);
     if (m->opt_engine == 2) { set_error("tensor-core engine forced but not usable for this model/batch/n_neighbors"); return TCSDN_EINVAL; }
     return launch_knn_exact_kneighbors(m, x, n, dtype, nn, ind, dist, flag, st);
 }
@@ -303,7 +303,7 @@ int tcsdn_knn_create_weighted(const double *fit_x, const int32_t *y, int64_t n_t
     m->n_train = n_train; m->k = k; m->knn_weights = weights;
     int r = upload(&m->d_fit, fit_x, (size_t)n_train * d);
     if (r == TCSDN_OK) r = upload(&m->d_y, y, (size_t)n_train);
-    if (r == TCSDN_OK) r = engine_create(m);
+    if (r == TCSDN_OK) r = knn_engine_create(m);
     if (r != TCSDN_OK) { tcsdn_destroy(m); return r; }
     *out = m;
     return TCSDN_OK;
@@ -338,7 +338,7 @@ int tcsdn_svc_create(const double *sv, const double *dual_coef, const double *in
     if (r == TCSDN_OK) r = upload(&m->d_coef, dual_coef, (size_t)(n_classes - 1) * n_sv);
     if (r == TCSDN_OK) r = upload(&m->d_rho, rho.data(), rho.size());
     if (r == TCSDN_OK) r = upload(&m->d_start, start.data(), start.size());
-    if (r == TCSDN_OK) r = engine_create(m);
+    if (r == TCSDN_OK) r = svc_engine_create(m);
     if (r != TCSDN_OK) { tcsdn_destroy(m); return r; }
     *out = m;
     return TCSDN_OK;

@@ -207,6 +207,35 @@ __device__ __forceinline__ void knn_weighted_vote(double *values, int32_t *indic
     }
 }
 
+// What a KNN kernel makes of a query's kept neighbours: the uniform vote (predict), the distance-weighted vote (predict on
+// weights='distance' handles) or the neighbours themselves (kneighbors)
+enum class KnnOut { Vote, WeightedVote, Neighbors };
+
+// Query q's result from its k kept neighbours (values / indices: squared distance and index, slot i at [i * ST]).  y maps an
+// index to its class, so it must match what the indices count: training labels for training indices, the engine's labels in
+// tile order for its tile positions (Vote only: the other two order equal distances by training index).
+//   Vote          labels[q] = the lowest class with the most neighbours; proba (nullable) [n][C] the class fractions
+//   WeightedVote  labels[q] and proba[q] (nullable) from knn_weighted_vote
+//   Neighbors     nb_ind [n][k] the indices and nb_dist [n][k] (nullable) the distances, by knn_write_neighbors
+template <KnnOut OUT, int ST>
+__device__ __forceinline__ void knn_finish(double *values, int32_t *indices, int k, int C, const int32_t *__restrict__ y, int64_t q,
+                                           int32_t *labels, double *proba, int64_t *nb_ind, double *nb_dist) {
+    if constexpr (OUT == KnnOut::Neighbors) {
+        knn_write_neighbors<ST>(values, indices, k, nb_ind + q * k, nb_dist ? nb_dist + q * k : nullptr);
+    } else if constexpr (OUT == KnnOut::WeightedVote) {
+        knn_weighted_vote<ST>(values, indices, k, C, y, labels + q, proba ? proba + q * C : nullptr);
+    } else {
+        int best = 0, arg = 0;
+        for (int c = 0; c < C; ++c) {
+            int votes = 0;
+            for (int i = 0; i < k; ++i) votes += (y[indices[i * ST]] == c);
+            if (proba) proba[q * C + c] = (double)votes / (double)k;
+            if (votes > best) { best = votes; arg = c; }
+        }
+        labels[q] = arg;
+    }
+}
+
 struct DeviceBuf {
     void *p = nullptr;
     size_t bytes = 0;
@@ -312,8 +341,10 @@ int launch_flow_update(double *state, const double *packets, const double *bytes
 int forest_pack(tcsdn_model *m, const int64_t *tree_offsets, const int32_t *left, const int32_t *right,
                 const int32_t *feature, const double *threshold, const double *value, int n_trees, int C);
 
-// tensor-core distance engine (dist_engine.cu)
-int engine_create(tcsdn_model *m);   // builds packed operands for knn / svc handles
+// tensor-core distance engine (dist_engine.cu).  The create functions build the packed operands; the state is attached to the
+// handle before anything is allocated, so that on an error return tcsdn_destroy frees what was made.
+int knn_engine_create(tcsdn_model *m);
+int svc_engine_create(tcsdn_model *m);
 void engine_destroy(tcsdn_model *m);
 bool engine_usable(const tcsdn_model *m, int64_t n, bool want_scores);
 void engine_read_stats(const tcsdn_model *m, int64_t *out8);
@@ -321,11 +352,13 @@ void engine_read_stats(const tcsdn_model *m, int64_t *out8);
 // `counter` (device) receives the number of such rows
 int launch_svc_marked(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, unsigned long long *counter,
                       cudaStream_t st);
-int launch_engine(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, double *scores,
-                  int32_t *flag, cudaStream_t st);
+int launch_knn_engine(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, double *scores,
+                      int32_t *flag, cudaStream_t st);
+int launch_svc_engine(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, double *scores,
+                      int32_t *flag, cudaStream_t st);
 bool engine_kneighbors_usable(const tcsdn_model *m, int64_t n, int nn);
-int launch_engine_kneighbors(tcsdn_model *m, const void *x, int64_t n, int dtype, int nn, int64_t *ind, double *dist,
-                             int32_t *flag, cudaStream_t st);
+int launch_knn_engine_kneighbors(tcsdn_model *m, const void *x, int64_t n, int dtype, int nn, int64_t *ind, double *dist,
+                                 int32_t *flag, cudaStream_t st);
 
 template <typename T>
 int upload(T **dst, const T *src, size_t count) {

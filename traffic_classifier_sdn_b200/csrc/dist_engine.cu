@@ -1,4 +1,5 @@
-// dist_engine.cu -- tensor-core (Hopper wgmma) distance engine shared by KNeighbors and SVC(rbf).
+// dist_engine.cu -- tensor-core (Hopper wgmma) distance engine of KNeighbors and SVC(rbf): one pipeline core (operand
+// packing, wgmma, shared-memory ring), two kernels, knn_engine_kernel and svc_engine_kernel.
 //
 // Both estimators need, for every (query row x, reference row t) pair, the squared euclidean distance
 //   d(x,t) = ||x||^2 + ||t||^2 - 2 x.t          (reference rows = training rows / support vectors)
@@ -27,8 +28,8 @@
 // k-th distance: there sklearn's answer depends on its heap's history.  The epilogue watches for rows left out at exactly the
 // final k-th distance; if such a row and the kept rows at that distance do not all carry one class, the query goes to the
 // index-order fp64 kernel (knn.cu, marked mode) in the same call; otherwise every choice gives the same class counts.
-// kneighbors (NC1 bit 2) returns the SET, so there any row left out at the final k-th distance sends the query to that kernel.
-// The distance-weighted vote (NC1 bit 3, weights='distance') keeps the class rule: equally distant rows weigh the same, so
+// kneighbors (KnnOut::Neighbors) returns the SET, so there any row left out at the final k-th distance sends the query to that
+// kernel.  The distance-weighted vote (KnnOut::WeightedVote) keeps the class rule: equally distant rows weigh the same, so
 // where every tied row carries one class, every choice gives the same (weight, class) columns in canonical order.
 // SVC uses acc directly, for LABELS only: e = -gamma log2(e) (acc + ||x' - c'_j||^2), K = ex2(e), C-1 fp32 FMAs per pair into
 // the running sums of the support vector's class, tile sums promoted to fp64.  To keep the fp32 accumulation error small
@@ -70,14 +71,15 @@
 // distance (n_tiles^2 x 2 B, 1.2 MB at 782 tiles; models beyond 4096 tiles walk outwards from the home tile in kd order and
 // test every tile).
 //
-// Kernel (persistent, 1 CTA / SM, 256 query rows per pass = two query tiles of 128 rows in the A operand, same canonical
+// Kernels (persistent, 1 CTA / SM, 256 query rows per pass = two query tiles of 128 rows in the A operand, same canonical
 // layout).  The epilogue warps form warpgroups; a warpgroup issues the wgmma itself (M64 N64 K16, 5 K steps per 64-row half
 // of a query tile, A and B from shared memory, fp32 accumulators in registers), waits for it, and every warp then transposes
 // its accumulator fragment through a private shared-memory buffer so that each thread sees whole accumulator rows:
-//   KNN: warps 0-7 (two warpgroups, one query tile each), each thread owns ONE query row: packs it into the A operand
-//               and runs the filter epilogue on the 64 columns of each reference tile;
-//   SVC: warps 0-3 (one warpgroup, both query tiles), each thread owns TWO query rows (one per query tile), so that one
-//               broadcast LDS.128 of dual coefficients feeds two rows;
+//   knn_engine_kernel: warps 0-7 (two warpgroups, one query tile each), each thread owns ONE query row: packs it into
+//               the A operand and runs the filter epilogue on the 64 columns of each reference tile.  Its variants: the
+//               heaps in shared or local memory, the audit, and the output (KnnOut: vote, weighted vote, neighbours);
+//   svc_engine_kernel: warps 0-3 (one warpgroup, both query tiles), each thread owns TWO query rows (one per query tile),
+//               so that one broadcast LDS.128 of dual coefficients feeds two rows; instantiated per class count and audit;
 //   last warp   streams reference tile images through a 4-stage ring (bulk copy + mbarrier tx count); SVC: every tile in
 //               order, one lane; KNN: the whole warp computes which tiles the pass needs (see above), lane 0 loads them.
 // Thread t of warp w owns row 64 (t >> 4) + 16 (w & 3) + (t & 15) of its query tile: exactly the rows of the warp's share of
@@ -95,7 +97,6 @@
 #include <algorithm>
 #include <cfloat>
 #include <cmath>
-#include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <type_traits>
@@ -109,8 +110,8 @@ constexpr int kEKnnWarps = 8;        // KNN epilogue warps (one query row per th
 constexpr int kESvcWarps = 4;        // SVC epilogue warps (two query rows per thread)
 constexpr int kEKnnThreads = (kEKnnWarps + 1) * 32;   // + producer warp
 constexpr int kESvcThreads = (kESvcWarps + 1) * 32;
-constexpr int kERows = 256;          // SVC: query rows per CTA pass (2 query tiles of 128)
-constexpr int kKnnRows = 256;        // KNN: query rows per CTA pass (2 query tiles of 128)
+constexpr int kEQTiles = 2;          // query tiles of 128 rows per CTA pass
+constexpr int kERows = kEQTiles * 128;   // query rows per CTA pass
 constexpr int kETStride = 68;        // row stride (floats) of the per-warp accumulator transpose buffer: 16-byte aligned rows
 constexpr int kETBytes = 8 * 32 * kETStride * 4;   // transpose buffers: KNN 8 warps x 32 rows, SVC 4 warps x 64 rows
 constexpr int kEN = 64;              // reference rows per tile (MMA N)
@@ -133,18 +134,23 @@ constexpr int kEMaxLeaves = 12000;           // KNN: kd leaves = bins of the que
 constexpr int kEMaxPruneTiles = 4096;        // KNN: the tile-by-tile neighbour table is n_tiles^2 x 2 bytes; larger models visit every tile
 constexpr int kEFlushTiles = 31;            // default number of reference tiles between two evaluation rounds (KNN), <= 31
 
+// Device state of an engine (m->engine): what both kinds keep, then each kind's own
 struct EngineState {
     unsigned char *d_tiles = nullptr;   // tile images
-    int32_t *d_tile_class = nullptr;    // per tile: class id (SVC)
-    int32_t *d_tile_row0 = nullptr;     // per tile: index of its first reference row in the ORIGINAL order
-    int32_t *d_tile_rows = nullptr;     // per tile: number of real rows
     double *d_center = nullptr;         // [d]
-    double *d_refpad = nullptr;         // KNN: original fp64 reference rows, row stride padded to an even count (16 B loads)
     float *d_maxratio = nullptr;        // audit: max observed |acc - exact| / (||x||^2 + ||t||^2)  (SVC: / M_j)
     unsigned long long *d_counters = nullptr;  // [0] exact re-evaluations (KNN) / rows handed to the fp64 kernel (SVC),
                                                // [1] KNN rows re-run in index order (class-relevant tie at the k-th distance),
                                                // [2] KNN reference tiles multiplied (summed over passes), [3] KNN passes
-    // KNN pruning (see "KNN: spatial order and pruning" in the file header)
+    int n_tiles = 0;
+    int tile_bytes = 0;
+    ~EngineState();                     // frees the device buffers
+};
+
+struct KnnEngine : EngineState {
+    int32_t *d_tile_rows = nullptr;     // per tile: number of real rows
+    double *d_refpad = nullptr;         // training rows in tile order, row stride padded to kEMaxD doubles (16 B loads)
+    // pruning (see "KNN: spatial order and pruning" in the file header)
     int32_t *d_kd_dim = nullptr;        // kd tree over the training rows: split coordinate per node, -1 = leaf
     int32_t *d_kd_child = nullptr;      // [node][2]: children; a leaf keeps its number in [node][0]
     double *d_kd_split = nullptr;       // split value (rows with x[dim] < split go left)
@@ -155,51 +161,61 @@ struct EngineState {
     uint16_t *d_nbr = nullptr;          // [n_tiles][n_tiles]: per home tile, all tiles by centre distance (nullptr: pruning off)
     float *d_chunk_lb = nullptr;        // [n_tiles][n_chunks]: min over positions >= 32 c of (centre distance - radius)
     int32_t *d_ypos = nullptr;          // training labels in tile order
-    int32_t *d_pos_orig = nullptr;      // KNN: tile position -> training index ([n_tiles * 64]; padding positions -1)
+    int32_t *d_pos_orig = nullptr;      // tile position -> training index ([n_tiles * 64]; padding positions -1)
     float *d_tile_tn = nullptr;         // per tile: largest ||t - c0||^2 of its rows (rounded up)
     cudaMemPool_t pool = nullptr;       // per-call scratch (query keys, permutation, tie list): stream-ordered allocations
-    int n_tiles = 0;
-    int tile_bytes = 0;
-    int nc1 = 0;
-    bool certifiable = true;            // SVC: the dual coefficients have libsvm's sign pattern (see the file header)
-    float eabs[(kEMaxNC1 + 1) * kEMaxNC1 / 2] = {};   // SVC: per pair, the absolute part of the bound
+    ~KnnEngine();
 };
 
+struct SvcEngine : EngineState {
+    int32_t *d_tile_class = nullptr;    // per tile: class id
+    int nc1 = 0;
+    bool certifiable = true;            // the dual coefficients have libsvm's sign pattern (see the file header)
+    float eabs[(kEMaxNC1 + 1) * kEMaxNC1 / 2] = {};   // per pair, the absolute part of the bound
+    ~SvcEngine();
+};
+
+// Kernel arguments: what both kernels read, then each kind's own
 struct EngineArgs {
     const unsigned char *tiles;
-    const int32_t *tile_class;
-    const int32_t *tile_row0;
-    const int32_t *tile_rows;
     const double *center;
-    const double *ref;       // original fp64 reference rows (audit statistic)
-    const double *refpad;    // the same rows at a 16-byte-aligned stride of dpad doubles (KNN exact re-evaluation)
-    const int32_t *y;        // KNN labels (original order: the distance-weighted vote reads them by training index)
-    const int32_t *ypos;     // KNN labels in tile order
-    const int32_t *qperm;    // KNN: this call's query order (sorted by home tile) or nullptr = as given
-    const int32_t *qkey;     // KNN: kd leaf per query (by original index)
-    const int32_t *leaf_tile;
-    const double *tcent;     // KNN: tile centres / radii
-    const double *trad;
-    const uint16_t *nbr;     // KNN: tiles by centre distance per home tile; nullptr = walk outwards from the home tile in kd order
-    const float *chunk_lb;
-    const float *tile_tn;    // KNN: per tile, the largest centred squared norm of its rows
-    int32_t *tie_list;       // KNN: rows whose label needs the index-order heap (ties at the k-th distance across classes)
-    int *tie_count;
-    const double *rho;       // SVC
     float *maxratio;         // non-null = audit mode
     int32_t *flag;
     int64_t n;
-    int n_tiles, tile_bytes, d, dpad, k, C, nc1, flush_tiles, n_ref;
-    int svc_mode;            // SVC: 0 = labels, uncertified rows stored as -1 - label; 3 = raw labels + decision values in
-                             // scores (audit, also records the MMA error ratio); 4 = raw labels + the bounds E_p in scores
-    float g2;                // SVC: -gamma * log2(e)
-    float svc_c1, svc_c2;    // SVC: gamma (2^-20 + 2^-24) and gamma 2^-24, the row-dependent parts of eta_j
-    float svc_eabs[(kEMaxNC1 + 1) * kEMaxNC1 / 2];   // SVC: per pair, the absolute part of E_p (file header)
-    // KNN kneighbors instantiations (NC1 bit 2): k is the call's n_neighbors; per row, the kept training indices (int64) and,
-    // when nb_dist is non-null, their distances, [n][k] in ascending (distance, index) order
+    int n_tiles, tile_bytes, d;
+};
+
+struct KnnArgs : EngineArgs {
+    const int32_t *tile_rows;
+    const double *refpad;    // training rows in tile order at a 16-byte-aligned stride of dpad doubles (exact re-evaluation)
+    const int32_t *y;        // labels by training index (the neighbours and the distance-weighted vote)
+    const int32_t *ypos;     // labels in tile order
+    const int32_t *qperm;    // this call's query order (sorted by home tile) or nullptr = as given
+    const int32_t *qkey;     // kd leaf per query (by original index)
+    const int32_t *leaf_tile;
+    const double *tcent;     // tile centres / radii
+    const double *trad;
+    const uint16_t *nbr;     // tiles by centre distance per home tile; nullptr = walk outwards from the home tile in kd order
+    const float *chunk_lb;
+    const float *tile_tn;    // per tile, the largest centred squared norm of its rows
+    int32_t *tie_list;       // rows whose result needs the index-order heap (ties at the k-th distance)
+    int *tie_count;
+    int dpad, k, C, flush_tiles;
+    // KnnOut::Neighbors: k is the call's n_neighbors; per row, the kept training indices (int64) and, when nb_dist is
+    // non-null, their distances, [n][k] in ascending (distance, index) order
     const int32_t *pos_orig; // tile position -> training index
     int64_t *nb_ind;
     double *nb_dist;
+};
+
+struct SvcArgs : EngineArgs {
+    const int32_t *tile_class;
+    const double *rho;
+    int svc_mode;            // 0 = labels, uncertified rows stored as -1 - label; 3 = raw labels + decision values in
+                             // scores (audit, also records the MMA error ratio); 4 = raw labels + the bounds E_p in scores
+    float g2;                // -gamma * log2(e)
+    float svc_c1, svc_c2;    // gamma (2^-20 + 2^-24) and gamma 2^-24, the row-dependent parts of eta_j
+    float svc_eabs[(kEMaxNC1 + 1) * kEMaxNC1 / 2];   // per pair, the absolute part of E_p (file header)
 };
 
 // ------------------------------------------------------------------------------------------------ PTX helpers
@@ -459,7 +475,7 @@ __global__ void __launch_bounds__(kSortThreads) knn_scatter_kernel(const int32_t
     for (int64_t i = lo + threadIdx.x; i < hi; i += kSortThreads) perm[atomicAdd(&s_cur[key[i]], 1)] = (int32_t)i;
 }
 
-// ------------------------------------------------------------------------------------------------ the kernel
+// ------------------------------------------------------------------------------------------------ the kernels
 // Load one query row, centre it on c0, round to fp32 (x'), split -2 x' into three bf16 pieces and write the row of the A
 // operand (query tile qt, row rt).  Returns ||x'||^2 (fp64); xp receives x' (zeros for a dead row).
 template <typename T, bool SVC>
@@ -494,19 +510,6 @@ __device__ __forceinline__ double e_pack_row(const EngineArgs &A, const T *__res
     return qn;
 }
 
-// experiment build (-DTCSDN_EXP_KNN_TIMING, tools/ only): cycles spent per role and phase, summed into counters[8 ..]
-#if defined(TCSDN_EXP_KNN_TIMING)
-#define KT_DECL long long kt_t0 = 0; long long kt_acc[8] = {0, 0, 0, 0, 0, 0, 0, 0}
-#define KT_START() kt_t0 = clock64()
-#define KT_STOP(i) kt_acc[i] += clock64() - kt_t0
-#define KT_FLUSH(base, cond) if (cond) { for (int kt_i = 0; kt_i < 8; ++kt_i) atomicAdd(counters + 8 + (base) + kt_i, (unsigned long long)kt_acc[kt_i]); }
-#else
-#define KT_DECL
-#define KT_START()
-#define KT_STOP(i)
-#define KT_FLUSH(base, cond)
-#endif
-
 // KNN: what the producer and the epilogue warps tell each other about the tiles of a pass
 constexpr int kEBarRegion = 3072;   // barriers (256 B) + KnnShared
 struct KnnShared {
@@ -519,195 +522,186 @@ struct KnnShared {
 };
 static_assert(sizeof(KnnShared) + 256 <= kEBarRegion, "KnnShared does not fit");
 
-// AUDIT (SVC; KNN keeps its audit flag in NC1): a separate instantiation, because the audit indexes the accumulator registers
-// and x' dynamically, which would put them in local memory in the production kernel too
-template <typename T, bool SVC, int NC1, bool AUDIT = false>
-__global__ void __launch_bounds__(SVC ? kESvcThreads : kEKnnThreads, 1)
-engine_kernel(const __grid_constant__ EngineArgs A, const T *__restrict__ X, int32_t *__restrict__ labels,
-              double *__restrict__ scores, unsigned long long *__restrict__ counters) {
-    constexpr int kEpi = SVC ? kESvcWarps : kEKnnWarps;   // epilogue warps (whole warpgroups); then the producer warp
-    constexpr int kRows = SVC ? kERows : kKnnRows;        // query rows per pass
-    constexpr int kQT = kRows / 128;                      // query tiles of 128 rows
-    constexpr int kSt = kEStages;                         // ring depth
-    static_assert(kEpi % 4 == 0 && kEpi * 32 * (SVC ? 2 : 1) == kRows, "one query row per thread (SVC: two), whole warpgroups");
+// Shared memory of both kernels: the A operand (two query tiles), the per-warp accumulator transpose buffers, the ring of
+// kEStages tile images, then kEBarRegion bytes that start with the barriers (fullB, emptyB, aFull; SVC adds coefFree, KNN
+// keeps KnnShared at +256), then the kind's own data (`tail`).
+struct ESmem {
+    unsigned char *sA, *sB, *tail;
+    float *sT;
+    uint64_t *fullB, *emptyB, *aFull;
+};
+__device__ __forceinline__ ESmem e_carve(unsigned char *smem, int tile_bytes) {
+    ESmem S;
+    S.sA = smem;                                                   // kEQTiles x kEATile
+    S.sT = reinterpret_cast<float *>(smem + kEQTiles * kEATile);   // kETBytes
+    S.sB = smem + kEQTiles * kEATile + kETBytes;                   // kEStages x tile_bytes
+    S.fullB = reinterpret_cast<uint64_t *>(S.sB + (size_t)kEStages * tile_bytes);
+    S.emptyB = S.fullB + kEStages;
+    S.aFull = S.emptyB + kEStages;
+    S.tail = reinterpret_cast<unsigned char *>(S.fullB) + kEBarRegion;
+    return S;
+}
+static size_t e_smem_bytes(int tile_bytes) {   // everything before `tail`
+    return (size_t)kEQTiles * kEATile + kETBytes + (size_t)kEStages * tile_bytes + kEBarRegion;
+}
+// thread 0: the ring's barriers and aFull (the pass's rows are packed), completed by the arrivals of the n_epi epilogue warps
+__device__ __forceinline__ void e_init_ring(const ESmem &S, int n_epi) {
+    for (int s = 0; s < kEStages; ++s) {
+        e_mbar_init(&S.fullB[s], 1);
+        e_mbar_init(&S.emptyB[s], n_epi);   // every epilogue warp's wgmma has read the stage
+    }
+    e_mbar_init(S.aFull, n_epi);
+}
+
+// KNN: the producer warp picks and streams the tiles of every pass; 8 epilogue warps (two warpgroups, one query tile each),
+// one query row per thread: pack A, wgmma, filter, deferred exact heap.  HEAP_SMEM: the k-slot heaps live in shared memory
+// (k <= kEHeapSmemK), else in thread-private local memory.  AUDIT: every pair passes the filter and the error statistic is
+// recorded.  OUT: what the kept neighbours become (knn_finish).
+template <typename T, bool HEAP_SMEM, bool AUDIT, KnnOut OUT>
+__global__ void __launch_bounds__(kEKnnThreads, 1)
+knn_engine_kernel(const __grid_constant__ KnnArgs A, const T *__restrict__ X, int32_t *__restrict__ labels,
+                  double *__restrict__ scores, unsigned long long *__restrict__ counters) {
+    static_assert(!AUDIT || OUT == KnnOut::Vote, "the audit is a mode of the vote");
+    constexpr int kRows = kERows;
+    constexpr int kSt = kEStages;
+    static_assert(kEKnnWarps % 4 == 0 && kEKnnWarps * 32 == kRows, "one query row per thread, whole warpgroups");
     extern __shared__ __align__(1024) unsigned char smem[];
-    unsigned char *sA = smem;                                          // kQT x 20480
-    float *sT = reinterpret_cast<float *>(smem + kQT * kEATile);       // kETBytes: per-warp accumulator transpose buffers
-    unsigned char *sB = smem + kQT * kEATile + kETBytes;               // kSt x tile_bytes
-    uint64_t *bars = reinterpret_cast<uint64_t *>(sB + (size_t)kSt * A.tile_bytes);
-    uint64_t *fullB = bars, *emptyB = bars + kEStages;
-    uint64_t *aFull = emptyB + kEStages;
-    uint64_t *coefFree = aFull + 1;      // the epilogue warps are done with a stage's side data (SVC coefficients)
-    // after the barriers -- KNN: [256 threads][kEListCap] candidate lists, then the heaps; SVC: [P][256] fp64 pair sums,
-    // then [P][256] fp32 error bounds
-    unsigned char *cand = reinterpret_cast<unsigned char *>(bars) + kEBarRegion;
-    KnnShared *ks = reinterpret_cast<KnnShared *>(reinterpret_cast<unsigned char *>(bars) + 256);   // KNN only
+    const ESmem S = e_carve(smem, A.tile_bytes);
+    KnnShared *ks = reinterpret_cast<KnnShared *>(reinterpret_cast<unsigned char *>(S.fullB) + 256);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int64_t n_super = (A.n + kRows - 1) / kRows;
-    // epilogue threads: the row of its query tile(s) this thread owns (see the file header) and its warp's transpose buffer
+    // epilogue threads: the row of its query tile this thread owns (see the file header) and its warp's transpose buffer
     const int rt = 64 * (lane >> 4) + 16 * (warp & 3) + (lane & 15);
-    float *tbuf = sT + (size_t)warp * (kRows / kEpi) * kETStride;
+    float *tbuf = S.sT + (size_t)warp * (kRows / kEKnnWarps) * kETStride;
 
     if (tid == 0) {
-        for (int s = 0; s < kEStages; ++s) {
-            e_mbar_init(&fullB[s], 1);
-            e_mbar_init(&emptyB[s], kEpi);     // every epilogue warp's wgmma has read the stage
-            e_mbar_init(&coefFree[s], kEpi);   // every epilogue warp has read the stage's side data
-        }
-        e_mbar_init(aFull, kEpi);
-        if constexpr (!SVC) { ks->rho_bits[0] = 0u; ks->rho_bits[1] = 0u; }
+        e_init_ring(S, kEKnnWarps);
+        ks->rho_bits[0] = 0u; ks->rho_bits[1] = 0u;
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
 
-    if (warp == kEpi) {
+    if (warp == kEKnnWarps) {
         // ------------------------------------------------------------------ reference tile producer
-        if constexpr (SVC) {
-            if (lane == 0) {
-                uint32_t g = 0;
-                for (int64_t st = blockIdx.x; st < n_super; st += gridDim.x) {
-                    for (int j = 0; j < A.n_tiles; ++j, ++g) {
-                        const uint32_t s = g % kEStages, ph = (g / kEStages) & 1;
-                        e_mbar_wait(&emptyB[s], ph ^ 1);
-                        e_mbar_wait(&coefFree[s], ph ^ 1);   // the epilogue warps are done with the stage's coefficients
-                        e_mbar_expect_tx(&fullB[s], (uint32_t)A.tile_bytes);
-                        e_bulk_g2s(sB + (size_t)s * A.tile_bytes, A.tiles + (size_t)j * A.tile_bytes, (uint32_t)A.tile_bytes, &fullB[s]);
-                    }
+        // KNN: per pass, the tiles in the order of their centres' distance from the pass's home tile, each tested against
+        //   (||x0 - c_t|| - r_t - rho)^2 > H   =>  no row of tile t can enter the neighbour set of any row of the pass
+        // (x0 = first row of the pass, rho = largest ||x - x0|| in the pass, H = largest current k-th distance^2 in the pass;
+        // H only falls, so a test that passes with a stale H stays valid).  Lanes compute the 32 gaps of a chunk in fp64, lane 0
+        // walks the chunk with the current H and loads what survives; a chunk-level bound ends the pass early.
+        const bool prune = A.qperm != nullptr;
+        const int n_chunks = (A.n_tiles + 31) >> 5;
+        uint32_t g = 0, pass = 0;            // g is lane 0's
+        unsigned long long n_mult = 0;
+        for (int64_t st = blockIdx.x; st < n_super; st += gridDim.x, ++pass) {
+            e_mbar_poll(S.aFull, pass & 1);    // the pass's rows are packed, rho is known
+            const int64_t src0 = A.qperm ? (int64_t)A.qperm[st * kRows] : st * kRows;
+            int home = 0;
+            float rho = 0.f, base_up = 0.f;
+            double x0[kEMaxD];
+            if (prune) {
+                home = A.leaf_tile[A.qkey[src0]];
+                rho = __uint_as_float(*reinterpret_cast<volatile unsigned *>(&ks->rho_bits[pass & 1]));
+                double dh = 0.0;
+#pragma unroll
+                for (int jj = 0; jj < kEMaxD; ++jj) {
+                    x0[jj] = jj < A.d ? static_cast<double>(X[src0 * A.d + jj]) : 0.0;
+                    const double df = jj < A.d ? x0[jj] - A.tcent[(size_t)home * A.d + jj] : 0.0;
+                    dh += df * df;
                 }
+                base_up = __fadd_ru(__double2float_ru(sqrt(dh) * (1.0 + 1e-12)), rho);   // >= ||q - c_home|| for every row q of the pass
             }
-        } else {
-            // KNN: per pass, the tiles in the order of their centres' distance from the pass's home tile, each tested against
-            //   (||x0 - c_t|| - r_t - rho)^2 > H   =>  no row of tile t can enter the neighbour set of any row of the pass
-            // (x0 = first row of the pass, rho = largest ||x - x0|| in the pass, H = largest current k-th distance^2 in the pass;
-            // H only falls, so a test that passes with a stale H stays valid).  Lanes compute the 32 gaps of a chunk in fp64, lane 0
-            // walks the chunk with the current H and loads what survives; a chunk-level bound ends the pass early.
-            const bool prune = A.qperm != nullptr;
-            const int n_chunks = (A.n_tiles + 31) >> 5;
-            uint32_t g = 0, pass = 0;            // g is lane 0's
-            unsigned long long n_mult = 0;
-            KT_DECL;
-            for (int64_t st = blockIdx.x; st < n_super; st += gridDim.x, ++pass) {
-                KT_START();
-                e_mbar_poll(aFull, pass & 1);    // the pass's rows are packed, rho is known
-                KT_STOP(0);
-                KT_START();
-                const int64_t src0 = A.qperm ? (int64_t)A.qperm[st * kRows] : st * kRows;
-                int home = 0;
-                float rho = 0.f, base_up = 0.f;
-                double x0[kEMaxD];
-                if (prune) {
-                    home = A.leaf_tile[A.qkey[src0]];
-                    rho = __uint_as_float(*reinterpret_cast<volatile unsigned *>(&ks->rho_bits[pass & 1]));
-                    double dh = 0.0;
+            auto current_h = [&]() {         // every lane: max over the epilogue warps
+                float h = lane < kEKnnWarps ? *reinterpret_cast<volatile float *>(&ks->warpH[lane]) : 0.f;
+#pragma unroll
+                for (int o = 16; o; o >>= 1) h = fmaxf(h, __shfl_xor_sync(0xffffffffu, h, o));
+                return h;
+            };
+            for (int c = 0; c < n_chunks; ++c) {
+                const float current_h_all = prune ? current_h() : 0.f;
+                if (prune && A.nbr) {        // everything from this chunk on is farther than H from every row of the pass
+                    const float mgn = __fsub_rd(A.chunk_lb[(size_t)home * n_chunks + c], base_up);
+                    if (mgn > 0.f && __fmul_rd(mgn, mgn) > current_h_all) break;
+                }
+                int t = c * 32 + lane;
+                const bool valid = t < A.n_tiles;
+                float gap = -FLT_MAX;
+                if (prune && valid) {
+                    if (A.nbr) {
+                        t = A.nbr[(size_t)home * A.n_tiles + t];
+                    } else {
+                        // no tile-by-tile table (models beyond kEMaxPruneTiles): neighbours in kd order are neighbours in
+                        // space, so walk outwards from the home tile -- home, +1, -1, +2, -2, ... then what is left of the
+                        // longer side; every tile is tested (no early end of the pass)
+                        const int lo = home, hi = A.n_tiles - 1 - home, mside = min(lo, hi);
+                        if (t <= 2 * mside) { const int kk = (t + 1) >> 1; t = (t & 1) ? home + kk : home - kk; }
+                        else { const int jj = t - 2 * mside; t = hi > lo ? home + mside + jj : home - mside - jj; }
+                    }
+                    double dd = 0.0;
 #pragma unroll
                     for (int jj = 0; jj < kEMaxD; ++jj) {
-                        x0[jj] = jj < A.d ? static_cast<double>(X[src0 * A.d + jj]) : 0.0;
-                        const double df = jj < A.d ? x0[jj] - A.tcent[(size_t)home * A.d + jj] : 0.0;
-                        dh += df * df;
+                        const double df = jj < A.d ? x0[jj] - A.tcent[(size_t)t * A.d + jj] : 0.0;
+                        dd += df * df;
                     }
-                    base_up = __fadd_ru(__double2float_ru(sqrt(dh) * (1.0 + 1e-12)), rho);   // >= ||q - c_home|| for every row q of the pass
+                    gap = __double2float_rd(sqrt(dd) * (1.0 - 1e-12) - A.trad[t]);   // <= ||x0 - row|| for every row of tile t
                 }
-                auto current_h = [&]() {         // every lane: max over the epilogue warps
-                    float h = lane < kEKnnWarps ? *reinterpret_cast<volatile float *>(&ks->warpH[lane]) : 0.f;
-#pragma unroll
-                    for (int o = 16; o; o >>= 1) h = fmaxf(h, __shfl_xor_sync(0xffffffffu, h, o));
-                    return h;
-                };
-                KT_STOP(1);
-                for (int c = 0; c < n_chunks; ++c) {
-                    KT_START();
-                    const float current_h_all = prune ? current_h() : 0.f;
-                    if (prune && A.nbr) {        // everything from this chunk on is farther than H from every row of the pass
-                        const float mgn = __fsub_rd(A.chunk_lb[(size_t)home * n_chunks + c], base_up);
-                        if (mgn > 0.f && __fmul_rd(mgn, mgn) > current_h_all) break;
-                    }
-                    int t = c * 32 + lane;
-                    const bool valid = t < A.n_tiles;
-                    float gap = -FLT_MAX;
-                    if (prune && valid) {
-                        if (A.nbr) {
-                            t = A.nbr[(size_t)home * A.n_tiles + t];
-                        } else {
-                            // no tile-by-tile table (models beyond kEMaxPruneTiles): neighbours in kd order are neighbours in
-                            // space, so walk outwards from the home tile -- home, +1, -1, +2, -2, ... then what is left of the
-                            // longer side; every tile is tested (no early end of the pass)
-                            const int lo = home, hi = A.n_tiles - 1 - home, mside = min(lo, hi);
-                            if (t <= 2 * mside) { const int kk = (t + 1) >> 1; t = (t & 1) ? home + kk : home - kk; }
-                            else { const int jj = t - 2 * mside; t = hi > lo ? home + mside + jj : home - mside - jj; }
-                        }
-                        double dd = 0.0;
-#pragma unroll
-                        for (int jj = 0; jj < kEMaxD; ++jj) {
-                            const double df = jj < A.d ? x0[jj] - A.tcent[(size_t)t * A.d + jj] : 0.0;
-                            dd += df * df;
-                        }
-                        gap = __double2float_rd(sqrt(dd) * (1.0 - 1e-12) - A.trad[t]);   // <= ||x0 - row|| for every row of tile t
-                    }
-                    // every lane tests its own tile against the H of this moment; lane 0 then walks the survivors in order and
-                    // tests each once more with the H of the moment it is loaded
-                    bool keep = valid;
-                    if (prune && valid) {
-                        const float mgn = __fsub_rd(gap, rho);
-                        keep = !(mgn > 0.f && __fmul_rd(mgn, mgn) > current_h_all);
-                    }
-                    unsigned todo = __ballot_sync(0xffffffffu, keep);
-                    ks->chunkT[lane] = t;
-                    ks->chunkGap[lane] = gap;
-                    __syncwarp();
-                    KT_STOP(2);
-                    if (lane == 0) {
-                        for (; todo; todo &= todo - 1) {
-                            const int i = __ffs(todo) - 1;
-                            const int ti = ks->chunkT[i];
-                            const float gi = ks->chunkGap[i];
-                            if (prune) {
-                                float h = 0.f;
-#pragma unroll
-                                for (int w = 0; w < kEKnnWarps; ++w) h = fmaxf(h, *reinterpret_cast<volatile float *>(&ks->warpH[w]));
-                                const float mgn = __fsub_rd(gi, rho);
-                                if (mgn > 0.f && __fmul_rd(mgn, mgn) > h) continue;
-                            }
-                            const uint32_t s = g % kSt, ph = (g / kSt) & 1;
-                            KT_START();
-                            e_mbar_poll(&emptyB[s], ph ^ 1);
-                            KT_STOP(3);
-                            e_sts_v2(&ks->stageInfo[s], make_int2(ti, __float_as_int(gi)));
-                            e_mbar_expect_tx(&fullB[s], (uint32_t)A.tile_bytes);
-                            e_bulk_g2s(sB + (size_t)s * A.tile_bytes, A.tiles + (size_t)ti * A.tile_bytes, (uint32_t)A.tile_bytes, &fullB[s]);
-                            ++g;
-                            ++n_mult;
-                        }
-                    }
-                    __syncwarp();
+                // every lane tests its own tile against the H of this moment; lane 0 then walks the survivors in order and
+                // tests each once more with the H of the moment it is loaded
+                bool keep = valid;
+                if (prune && valid) {
+                    const float mgn = __fsub_rd(gap, rho);
+                    keep = !(mgn > 0.f && __fmul_rd(mgn, mgn) > current_h_all);
                 }
-                if (lane == 0) {                 // end of pass: an empty stage that carries -1
-                    const uint32_t s = g % kSt, ph = (g / kSt) & 1;
-                    e_mbar_poll(&emptyB[s], ph ^ 1);
-                    e_sts_v2(&ks->stageInfo[s], make_int2(-1, 0));
-                    e_mbar_arrive(&fullB[s]);
-                    ++g;
+                unsigned todo = __ballot_sync(0xffffffffu, keep);
+                ks->chunkT[lane] = t;
+                ks->chunkGap[lane] = gap;
+                __syncwarp();
+                if (lane == 0) {
+                    for (; todo; todo &= todo - 1) {
+                        const int i = __ffs(todo) - 1;
+                        const int ti = ks->chunkT[i];
+                        const float gi = ks->chunkGap[i];
+                        if (prune) {
+                            float h = 0.f;
+#pragma unroll
+                            for (int w = 0; w < kEKnnWarps; ++w) h = fmaxf(h, *reinterpret_cast<volatile float *>(&ks->warpH[w]));
+                            const float mgn = __fsub_rd(gi, rho);
+                            if (mgn > 0.f && __fmul_rd(mgn, mgn) > h) continue;
+                        }
+                        const uint32_t s = g % kSt, ph = (g / kSt) & 1;
+                        e_mbar_poll(&S.emptyB[s], ph ^ 1);
+                        e_sts_v2(&ks->stageInfo[s], make_int2(ti, __float_as_int(gi)));
+                        e_mbar_expect_tx(&S.fullB[s], (uint32_t)A.tile_bytes);
+                        e_bulk_g2s(S.sB + (size_t)s * A.tile_bytes, A.tiles + (size_t)ti * A.tile_bytes, (uint32_t)A.tile_bytes, &S.fullB[s]);
+                        ++g;
+                        ++n_mult;
+                    }
                 }
                 __syncwarp();
             }
-            if (lane == 0 && counters) { atomicAdd(counters + 2, n_mult); atomicAdd(counters + 3, (unsigned long long)pass); }
-            KT_FLUSH(0, lane == 0 && counters);
+            if (lane == 0) {                 // end of pass: an empty stage that carries -1
+                const uint32_t s = g % kSt, ph = (g / kSt) & 1;
+                e_mbar_poll(&S.emptyB[s], ph ^ 1);
+                e_sts_v2(&ks->stageInfo[s], make_int2(-1, 0));
+                e_mbar_arrive(&S.fullB[s]);
+                ++g;
+            }
+            __syncwarp();
         }
-    } else if constexpr (!SVC) {
+        if (lane == 0 && counters) { atomicAdd(counters + 2, n_mult); atomicAdd(counters + 3, (unsigned long long)pass); }
+    } else {
         // ------------------------------------------------------------------ KNN: 256 query-row owners (pack A, wgmma, filter epilogue)
         const int qt = warp >> 2;                           // query tile 0..1 = this thread's warpgroup
         const bool prune = A.qperm != nullptr;
         uint32_t g = 0, pass = 0;
         float nf = 0.f;
-        KT_DECL;
         for (int64_t st = blockIdx.x; st < n_super; st += gridDim.x, ++pass) {
-            KT_START();
-            e_wg_sync(qt);                                  // the warpgroup's last wgmma of the previous pass has read sA
+            e_wg_sync(qt);                                  // the warpgroup's last wgmma of the previous pass has read S.sA
             const int64_t slot = st * kRows + qt * 128 + rt;
             const bool live = slot < A.n;
             const int64_t row = !live ? 0 : (A.qperm ? (int64_t)A.qperm[slot] : slot);   // the query this thread owns
             float xp_unused[kEMaxD];
-            const double qn = e_pack_row<T, false>(A, X, row, live, sA, qt, rt, nf, xp_unused);
+            const double qn = e_pack_row<T, false>(A, X, row, live, S.sA, qt, rt, nf, xp_unused);
             // distance from the pass's first row (the producer's reference point), rounded up; its maximum over the pass is rho
             float e_up = 0.f;
             if (prune) {
@@ -730,9 +724,8 @@ engine_kernel(const __grid_constant__ EngineArgs A, const T *__restrict__ X, int
             }
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to wgmma
             __syncwarp();
-            if (lane == 0) e_mbar_arrive(aFull);
+            if (lane == 0) e_mbar_arrive(S.aFull);
             e_wg_sync(qt);                                  // the query tile is complete
-            KT_STOP(0);
 
             {
                 // ================================================================ KNN: filter, deferred exact heap
@@ -748,25 +741,22 @@ engine_kernel(const __grid_constant__ EngineArgs A, const T *__restrict__ X, int
                 // or evicted while an equal value stays): if such a row and the kept rows at that distance do not all carry one
                 // class, the label depends on the choice and the row goes to the index-order fp64 kernel (tie_list); otherwise
                 // the class counts -- label and probabilities -- are the same for every choice.
-                // The k-slot max-heap: shared memory [slot][thread] for k <= 8 (NC1 bit 0), else thread-private local
+                // The k-slot max-heap: shared memory [slot][thread] for k <= 8 (HEAP_SMEM), else thread-private local
                 // memory.  Its root and the filter threshold stay in registers.
-                constexpr bool kHeapSmem = (NC1 & 1) != 0;      // KNN instantiations: NC1 bit 0 = heap in shared memory,
-                constexpr bool kAudit = (NC1 & 2) != 0;         //                     bit 1 = audit mode (error statistic),
-                constexpr bool kKnb = (NC1 & 4) != 0;           //                     bit 2 = kneighbors (rows of A.nb_ind / A.nb_dist),
-                constexpr bool kWd = (NC1 & 8) != 0;            //                     bit 3 = distance-weighted vote
-                constexpr int ST = kHeapSmem ? kKnnRows : 1;
-                double hv_local[kHeapSmem ? 1 : kEMaxK];
-                int32_t hi_local[kHeapSmem ? 1 : kEMaxK];
-                unsigned char *heap_base = cand + kKnnRows * kEListCap * sizeof(uint16_t);
-                double *hv = kHeapSmem ? reinterpret_cast<double *>(heap_base) + tid : hv_local;
-                int32_t *hi = kHeapSmem ? reinterpret_cast<int32_t *>(heap_base + kKnnRows * (size_t)A.k * sizeof(double)) + tid : hi_local;
+                constexpr bool kKnb = OUT == KnnOut::Neighbors;   // the output is the neighbour SET
+                constexpr int ST = HEAP_SMEM ? kERows : 1;
+                double hv_local[HEAP_SMEM ? 1 : kEMaxK];
+                int32_t hi_local[HEAP_SMEM ? 1 : kEMaxK];
+                unsigned char *heap_base = S.tail + kERows * kEListCap * sizeof(uint16_t);
+                double *hv = HEAP_SMEM ? reinterpret_cast<double *>(heap_base) + tid : hv_local;
+                int32_t *hi = HEAP_SMEM ? reinterpret_cast<int32_t *>(heap_base + kERows * (size_t)A.k * sizeof(double)) + tid : hi_local;
                 for (int i = 0; i < A.k; ++i) { hv[i * ST] = DBL_MAX; hi[i * ST] = 0; }
                 double hv0 = DBL_MAX, tie_val = -1.0;
                 int tie_cls = -1;
                 float thr_base = FLT_MAX, hv0f = __int_as_float(0x7f800000);
                 unsigned long long n_exact = 0;
                 // candidate list entries: sequence offset since the last round << 11 | group of 8 columns << 8 | pass mask
-                uint16_t *mylist = reinterpret_cast<uint16_t *>(cand) + (size_t)tid * kEListCap;
+                uint16_t *mylist = reinterpret_cast<uint16_t *>(S.tail) + (size_t)tid * kEListCap;
                 int32_t *myseq = ks->seqTile[warp];
                 int cnt = 0, base_seq = 0, next_round = 1, j = 0;
                 bool end = false;
@@ -790,7 +780,6 @@ engine_kernel(const __grid_constant__ EngineArgs A, const T *__restrict__ X, int
                     // fast), or when a list could overflow in this tile
                     const bool need = end || j >= next_round || cnt > kEListCap - kEListRoom;
                     if (__any_sync(0xffffffffu, need)) {
-                        KT_START();
                         int li = 0, gbase = 0;
                         uint32_t m = 0;
                         auto next = [&](int32_t &idx) -> bool {   // pops this thread's next candidate (position in tile order)
@@ -844,45 +833,40 @@ engine_kernel(const __grid_constant__ EngineArgs A, const T *__restrict__ X, int
                         base_seq = j;
                         // next round: after 1, 2, 4, 8, ... tiles while the threshold is still falling fast, then every flush_tiles tiles
                         next_round = j + min(A.flush_tiles, max(1, j));
-                        KT_STOP(1);
                     }
                     if (end) break;
                     // ---- the next tile of the pass (or its end)
                     const uint32_t s = g % kSt, ph = (g / kSt) & 1;
                     ++g;
-                    KT_START();
-                    e_mbar_poll(&fullB[s], ph);
-                    KT_STOP(2);
-                    KT_START();
+                    e_mbar_poll(&S.fullB[s], ph);
                     const int2 info = e_lds_v2(&ks->stageInfo[s]);
                     if (info.x < 0) {                       // end of pass (the branch on info also orders the load before the arrive)
                         __syncwarp();
-                        if (lane == 0) e_mbar_arrive(&emptyB[s]);
+                        if (lane == 0) e_mbar_arrive(&S.emptyB[s]);
                         end = true;
                         continue;
                     }
                     // the whole warpgroup multiplies its query tile by the reference tile (wgmma is warpgroup-collective, so no
                     // warp may skip it); once it has completed the stage goes back to the producer
-                    e_mma_tile(sA + qt * kEATile, sB + (size_t)s * A.tile_bytes, tbuf, lane);
-                    if (lane == 0) e_mbar_arrive(&emptyB[s]);
+                    e_mma_tile(S.sA + qt * kEATile, S.sB + (size_t)s * A.tile_bytes, tbuf, lane);
+                    if (lane == 0) e_mbar_arrive(&S.emptyB[s]);
                     // this row cannot gain a neighbour from the tile: ||x - t|| >= ||x0 - t|| - ||x - x0|| >= gap - e > sqrt(k-th distance^2)
                     const float mgn = __fsub_rd(__int_as_float(info.y), e_up);
-                    const bool far = !live || (!kAudit && prune && mgn > 0.f && __fmul_rd(mgn, mgn) > hv0f);
+                    const bool far = !live || (!AUDIT && prune && mgn > 0.f && __fmul_rd(mgn, mgn) > hv0f);
                     if (lane == 0) myseq[j - base_seq] = info.x;
                     if (__all_sync(0xffffffffu, far)) {     // nobody in the warp needs the tile: leave the accumulators unread
                         ++j;
-                        KT_STOP(3);
                         continue;
                     }
                     // ---- filter the tile: two halves of 32 accumulator columns (keeps 32, not 64, values live)
-                    float thr = far ? -FLT_MAX : (kAudit ? FLT_MAX : thr_base);
+                    float thr = far ? -FLT_MAX : (AUDIT ? FLT_MAX : thr_base);
                     const uint32_t etile = (uint32_t)(j - base_seq) << 11;
                     uint32_t lp = e_smem(mylist) + 2u * (uint32_t)cnt;   // 32-bit shared address of the list's tail
                     // this thread's accumulator row, all 64 values
                     uint32_t r0[32], r1[32];
                     e_ld_row(tbuf + lane * kETStride, r0);
                     e_ld_row(tbuf + lane * kETStride + 32, r1);
-                    if constexpr (kHeapSmem && !kAudit) {
+                    if constexpr (HEAP_SMEM && !AUDIT) {
                         // No threshold yet (the pass's first tile): instead of re-evaluating all 64 rows exactly, take the k-th
                         // smallest ACCUMULATOR value s: the k-th smallest exact distance of the tile is at most
                         //   U = s + ||x||^2 + 2 kappa (||x||^2 + TN)      (TN = the tile's largest ||t||^2; |acc - (d - ||x||^2 -
@@ -937,7 +921,7 @@ engine_kernel(const __grid_constant__ EngineArgs A, const T *__restrict__ X, int
                             for (int c = 0; c < 8; ++c) mask |= (v[gq * 8 + c] <= thr) ? (1u << c) : 0u;
                             if (mask) asm volatile("st.shared.u16 [%0], %1;" ::"r"(lp), "h"((uint16_t)(etile | (uint32_t)((h * 4 + gq) << 8) | mask)) : "memory");
                             lp += mask ? 2u : 0u;
-                            if constexpr (kAudit) {   // error statistic while the accumulator values are at hand
+                            if constexpr (AUDIT) {   // error statistic while the accumulator values are at hand
 #pragma unroll
                                 for (int c = 0; c < 8; ++c) {
                                     const int col = h * 32 + gq * 8 + c;
@@ -957,9 +941,7 @@ engine_kernel(const __grid_constant__ EngineArgs A, const T *__restrict__ X, int
                     }
                     cnt = (int)((lp - e_smem(mylist)) >> 1);
                     ++j;
-                    KT_STOP(4);
                 }
-                KT_START();
                 if (live) {
                     // a row outside the kept set at exactly the k-th distance: does the choice among the tied rows matter?  For
                     // the vote only if the tied rows' classes differ; for kneighbors always (the SET is the index-order heap's)
@@ -972,33 +954,64 @@ engine_kernel(const __grid_constant__ EngineArgs A, const T *__restrict__ X, int
                     if (tied) {
                         if constexpr (!kKnb) labels[row] = -1;
                         A.tie_list[atomicAdd(A.tie_count, 1)] = (int32_t)row;
-                    } else if constexpr (kKnb) {
-                        for (int i = 0; i < A.k; ++i) hi[i * ST] = A.pos_orig[hi[i * ST]];
-                        knn_write_neighbors<ST>(hv, hi, A.k, A.nb_ind + row * A.k, A.nb_dist ? A.nb_dist + row * A.k : nullptr);
-                    } else if constexpr (kWd) {
+                    } else if constexpr (OUT == KnnOut::Vote) {
+                        knn_finish<OUT, ST>(hv, hi, A.k, A.C, A.ypos, row, labels, scores, nullptr, nullptr);
+                    } else {
                         // equal distances are ordered by TRAINING index: map the tile positions before the sort
                         for (int i = 0; i < A.k; ++i) hi[i * ST] = A.pos_orig[hi[i * ST]];
-                        knn_weighted_vote<ST>(hv, hi, A.k, A.C, A.y, labels + row, scores ? scores + row * A.C : nullptr);
-                    } else {
-                        int best = 0, arg = 0;
-                        for (int c = 0; c < A.C; ++c) {
-                            int votes = 0;
-                            for (int i = 0; i < A.k; ++i) votes += (A.ypos[hi[i * ST]] == c);
-                            if (scores) scores[row * A.C + c] = (double)votes / (double)A.k;
-                            if (votes > best) { best = votes; arg = c; }
-                        }
-                        labels[row] = arg;
+                        knn_finish<OUT, ST>(hv, hi, A.k, A.C, A.y, row, labels, scores, A.nb_ind, A.nb_dist);
                     }
                 }
                 {   // one counter update per warp
                     const unsigned wsum = __reduce_add_sync(0xffffffffu, live ? (unsigned)n_exact : 0u);
                     if (lane == 0 && counters) atomicAdd(counters, (unsigned long long)wsum);
                 }
-                KT_STOP(5);
             }
         }
-        KT_FLUSH(16, lane == 0 && counters);
         if (A.flag && nf != nf) atomicOr(A.flag, 1);
+    }
+}
+
+// SVC(rbf): the producer's lane 0 streams every tile in order; 4 epilogue warps (one warpgroup, both query tiles), two query
+// rows per thread.  NC1 = n_classes - 1.  AUDIT: a separate instantiation, because the audit indexes the accumulator
+// registers and x' dynamically, which would put them in local memory in the production kernel too
+template <typename T, int NC1, bool AUDIT>
+__global__ void __launch_bounds__(kESvcThreads, 1)
+svc_engine_kernel(const __grid_constant__ SvcArgs A, const T *__restrict__ X, int32_t *__restrict__ labels,
+                  double *__restrict__ scores) {
+    constexpr int kRows = kERows;
+    static_assert(kESvcWarps % 4 == 0 && kESvcWarps * 64 == kRows, "two query rows per thread, whole warpgroups");
+    extern __shared__ __align__(1024) unsigned char smem[];
+    const ESmem S = e_carve(smem, A.tile_bytes);
+    uint64_t *coefFree = S.aFull + 1;    // the epilogue warps are done with a stage's side data (the coefficients)
+
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int64_t n_super = (A.n + kRows - 1) / kRows;
+    // epilogue threads: the row of the query tiles this thread owns (see the file header) and its warp's transpose buffer
+    const int rt = 64 * (lane >> 4) + 16 * (warp & 3) + (lane & 15);
+    float *tbuf = S.sT + (size_t)warp * (kRows / kESvcWarps) * kETStride;
+
+    if (tid == 0) {
+        e_init_ring(S, kESvcWarps);
+        for (int s = 0; s < kEStages; ++s) e_mbar_init(&coefFree[s], kESvcWarps);   // every epilogue warp has read the side data
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+
+    if (warp == kESvcWarps) {
+        // ------------------------------------------------------------------ reference tile producer
+        if (lane == 0) {
+            uint32_t g = 0;
+            for (int64_t st = blockIdx.x; st < n_super; st += gridDim.x) {
+                for (int j = 0; j < A.n_tiles; ++j, ++g) {
+                    const uint32_t s = g % kEStages, ph = (g / kEStages) & 1;
+                    e_mbar_wait(&S.emptyB[s], ph ^ 1);
+                    e_mbar_wait(&coefFree[s], ph ^ 1);   // the epilogue warps are done with the stage's coefficients
+                    e_mbar_expect_tx(&S.fullB[s], (uint32_t)A.tile_bytes);
+                    e_bulk_g2s(S.sB + (size_t)s * A.tile_bytes, A.tiles + (size_t)j * A.tile_bytes, (uint32_t)A.tile_bytes, &S.fullB[s]);
+                }
+            }
+        }
     } else {
         // ------------------------------------------------------------------ SVC: 4 warps x 2 query rows per thread
         // Every support-vector tile carries its own centre c'_j (tiles are spatially compact, see create()):
@@ -1006,14 +1019,14 @@ engine_kernel(const __grid_constant__ EngineArgs A, const T *__restrict__ X, int
         //   d   = ||x' - c'_j||^2 + acc ,  ||x' - c'_j||^2 summed directly in fp32 (no cancellation)
         // A thread owns row rt of BOTH query tiles, so one broadcast LDS.128 of coefficients serves both rows.
         constexpr int C = NC1 + 1, P = C * NC1 / 2;
-        double *decS = reinterpret_cast<double *>(cand);            // [P][256]: sum over finished classes of coef K
+        double *decS = reinterpret_cast<double *>(S.tail);            // [P][256]: sum over finished classes of coef K
         float *errS = reinterpret_cast<float *>(decS + P * kERows); // [P][256]: the matching error bound
         const int slot0 = rt;                                       // this thread's rows sit at slot0 and slot0 + 128
         const float g2 = A.g2;
         uint32_t g = 0;
         float nf = 0.f;
         for (int64_t st = blockIdx.x; st < n_super; st += gridDim.x) {
-            e_wg_sync(0);                                   // the last wgmma of the previous pass has read sA
+            e_wg_sync(0);                                   // the last wgmma of the previous pass has read S.sA
             int64_t row[2];
             bool live[2];
             float xp[2][kEMaxD], sq[2], c2row[2];
@@ -1021,7 +1034,7 @@ engine_kernel(const __grid_constant__ EngineArgs A, const T *__restrict__ X, int
             for (int r = 0; r < 2; ++r) {
                 row[r] = st * kERows + slot0 + r * 128;
                 live[r] = row[r] < A.n;
-                const double qn = e_pack_row<T, true>(A, X, row[r], live[r], sA, r, rt, nf, xp[r]);
+                const double qn = e_pack_row<T, true>(A, X, row[r], live[r], S.sA, r, rt, nf, xp[r]);
                 const float qnf = __double2float_ru(qn);
                 sq[r] = __fsqrt_ru(qnf);
                 c2row[r] = A.svc_c2 * qnf;
@@ -1030,7 +1043,7 @@ engine_kernel(const __grid_constant__ EngineArgs A, const T *__restrict__ X, int
             }
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to wgmma
             __syncwarp();
-            if (lane == 0) e_mbar_arrive(aFull);
+            if (lane == 0) e_mbar_arrive(S.aFull);
             e_wg_sync(0);                                   // both query tiles are complete
 
             // Per (row, coefficient row): FOUR fp32 partial sums per tile (even / odd columns x even / odd groups of four
@@ -1064,18 +1077,18 @@ engine_kernel(const __grid_constant__ EngineArgs A, const T *__restrict__ X, int
                 const int cls = A.tile_class[j];
                 if (cls != cur_class) { flush_class(cur_class); cur_class = cls; }   // uniform: support vectors are grouped by class
                 // the tile image (B operand, coefficients, header) was written by the bulk copy: observe its barrier
-                e_mbar_wait(&fullB[sidx], (g / kEStages) & 1);
+                e_mbar_wait(&S.fullB[sidx], (g / kEStages) & 1);
                 // both query tiles against the tile (warpgroup-collective); rows of query tile r land in rows [32 r, 32 r + 32)
                 // of the warp's transpose buffer
-                e_mma_tile(sA, sB + (size_t)sidx * A.tile_bytes, tbuf, lane);
-                e_mma_tile(sA + kEATile, sB + (size_t)sidx * A.tile_bytes, tbuf + 32 * kETStride, lane);
-                if (lane == 0) e_mbar_arrive(&emptyB[sidx]);
+                e_mma_tile(S.sA, S.sB + (size_t)sidx * A.tile_bytes, tbuf, lane);
+                e_mma_tile(S.sA + kEATile, S.sB + (size_t)sidx * A.tile_bytes, tbuf + 32 * kETStride, lane);
+                if (lane == 0) e_mbar_arrive(&S.emptyB[sidx]);
                 const float *trow0 = tbuf + lane * kETStride, *trow1 = trow0 + 32 * kETStride;
                 // accumulator columns are taken in chunks of 8 per row, double-buffered (32 registers)
                 uint32_t va0[8], va1[8], vb0[8], vb1[8];
                 e_ld_row(trow0, va0);
                 e_ld_row(trow1, va1);
-                const float *coef = reinterpret_cast<const float *>(sB + (size_t)sidx * A.tile_bytes + kETileB);
+                const float *coef = reinterpret_cast<const float *>(S.sB + (size_t)sidx * A.tile_bytes + kETileB);
                 const float4 *hdr = reinterpret_cast<const float4 *>(coef + NC1 * kEN);   // c'_j [12], eta constants
                 float xn[2] = {0.f, 0.f};   // ||x' - c'_j||^2 summed directly in fp32
 #pragma unroll
@@ -1121,11 +1134,7 @@ engine_kernel(const __grid_constant__ EngineArgs A, const T *__restrict__ X, int
                 auto load_cf = [&](float4 (&cf)[NA], int col) {
 #pragma unroll
                     for (int m = 0; m < NA; ++m)
-#if defined(TCSDN_EXP_NO_CFLDS)   // experiment build: no coefficient loads
-                        cf[m] = make_float4(0.5f, 0.25f, (float)(rowoff[m] + col), 1.f);
-#else
                         cf[m] = *reinterpret_cast<const float4 *>(coef + rowoff[m] + col);
-#endif
                 };
                 // exps of one block: K[r][0..3] for the two rows (two FFMA2 + four MUFU.EX2 per row)
                 struct K4 { float2 k01[2], k23[2]; };
@@ -1137,12 +1146,8 @@ engine_kernel(const __grid_constant__ EngineArgs A, const T *__restrict__ X, int
                         float2 e01 = bias2[r], e23 = bias2[r];
                         e_fma2(e01, make_float2(__uint_as_float(v[0]), __uint_as_float(v[1])), g22);
                         e_fma2(e23, make_float2(__uint_as_float(v[2]), __uint_as_float(v[3])), g22);
-#if defined(TCSDN_EXP_NO_EX2)   // experiment build (-DTCSDN_EXP_NO_EX2, never the product): no MUFU
-                        k.k01[r] = e01; k.k23[r] = e23;
-#else
                         k.k01[r] = make_float2(e_ex2(e01.x), e_ex2(e01.y));
                         k.k23[r] = make_float2(e_ex2(e23.x), e_ex2(e23.y));
-#endif
                     }
                     return k;
                 };
@@ -1176,7 +1181,7 @@ engine_kernel(const __grid_constant__ EngineArgs A, const T *__restrict__ X, int
                     uint32_t (&n1)[8] = (cc & 1) ? va1 : vb1;
                     if constexpr (AUDIT) {
                         // audit: |acc - exact| / M_j for this chunk's pairs -- exact from x' and the tile's packed fp32 pieces, in fp64
-                        const unsigned char *tb = sB + (size_t)sidx * A.tile_bytes;
+                        const unsigned char *tb = S.sB + (size_t)sidx * A.tile_bytes;
                         auto piece = [&](int rr, int k) { return (double)__bfloat162float(*reinterpret_cast<const __nv_bfloat16 *>(tb + tile_off(rr, k))); };
                         const float *cj = reinterpret_cast<const float *>(hdr);
                         double cn = 0.0;
@@ -1395,406 +1400,448 @@ static void pack_dummy(unsigned char *tile, int r, int d, bool inf) {
     memcpy(tile + tile_off(r, 6 * d + 0), &big, 2);
 }
 
-int engine_create(tcsdn_model *m) {
-    m->engine = nullptr;
-    const int d = m->d;
-    if (d > kEMaxD) return TCSDN_OK;                       // engine not applicable: fp64 kernels only
-    const bool svc = m->kind == TCSDN_KIND_SVC;
-    if (!svc && m->k > kEMaxK) return TCSDN_OK;
-    if (svc && m->n_classes - 1 > kEMaxNC1) return TCSDN_OK;
-    const int64_t nref = svc ? m->n_sv : m->n_train;
-    std::vector<double> ref((size_t)nref * d);
-    TCSDN_CUDA(cudaMemcpy(ref.data(), svc ? m->d_sv : m->d_fit, ref.size() * sizeof(double), cudaMemcpyDeviceToHost));
-    // Centre: the coordinate-wise median.  Any fixed point is correct; the tensor-core error scales with
-    // ||x-c||^2 + ||t-c||^2, and flow features are heavy-tailed (most rows sit near small values, a few classes reach
-    // 1e4..1e5): the median keeps the norms of the dense small-valued clusters small, the mean does not.
-    std::vector<double> center(d, 0.0), col((size_t)nref);
+// The reference rows (training rows / support vectors) on the host, and the centre c0 every row is taken relative to.
+// Centre: the coordinate-wise median.  Any fixed point is correct; the tensor-core error scales with
+// ||x-c||^2 + ||t-c||^2, and flow features are heavy-tailed (most rows sit near small values, a few classes reach
+// 1e4..1e5): the median keeps the norms of the dense small-valued clusters small, the mean does not.
+static int host_rows(const double *d_ref, int64_t nref, int d, std::vector<double> &ref, std::vector<double> &center) {
+    ref.resize((size_t)nref * d);
+    TCSDN_CUDA(cudaMemcpy(ref.data(), d_ref, ref.size() * sizeof(double), cudaMemcpyDeviceToHost));
+    center.assign(d, 0.0);
+    std::vector<double> col((size_t)nref);
     for (int j = 0; j < d; ++j) {
         for (int64_t i = 0; i < nref; ++i) col[(size_t)i] = ref[(size_t)i * d + j];
         std::nth_element(col.begin(), col.begin() + nref / 2, col.end());
         center[j] = col[(size_t)(nref / 2)];
     }
-
-    EngineState *E = new EngineState();
-    const int nc1 = svc ? m->n_classes - 1 : 0;
-    E->nc1 = nc1;
-    // tile image = bf16 B operand, then (SVC only) the tile's dual coefficients + centre
-    E->tile_bytes = kETileB + (svc ? nc1 * kEN * (int)sizeof(float) + 16 * (int)sizeof(float) : 0);
-    // tile plan: KNN = kd order (spatially compact tiles: whole tiles can be skipped, see the file header);
-    // SVC = per class (sums are per class), rows re-ordered inside the class for spatial compactness (sums do not
-    // care about order), padded to a tile boundary with zero-coefficient rows
-    std::vector<int32_t> row0, rows, tclass, order((size_t)nref);
-    std::vector<double> coef;          // SVC: dual coefficients [nc1][nref]
-    std::vector<uint8_t> pattern;      // SVC: per support vector, bit mm set iff coefficient row mm is non-zero
-    for (int64_t i = 0; i < nref; ++i) order[(size_t)i] = (int32_t)i;
-    KdTree kd;
-    if (!svc) {
-        while (kd.leaf_rows < kEN && nref / (kd.leaf_rows / 2 + 1) > kEMaxLeaves) kd.leaf_rows *= 2;   // the sort's histogram lives in shared memory
-        kd_build(ref, d, order, 0, (size_t)nref, kd);
-        for (int64_t r = 0; r < nref; r += kEN) { row0.push_back((int32_t)r); rows.push_back((int32_t)std::min<int64_t>(kEN, nref - r)); tclass.push_back(0); }
-    } else {
-        std::vector<int32_t> start(m->n_classes + 1);
-        TCSDN_CUDA(cudaMemcpy(start.data(), m->d_start, start.size() * sizeof(int32_t), cudaMemcpyDeviceToHost));
-        // inside a class: first by the vector's non-zero coefficient pattern (the kernel skips coefficient rows that are zero
-        // on a whole tile), then spatially compact inside every pattern group
-        coef.resize((size_t)nc1 * nref);
-        TCSDN_CUDA(cudaMemcpy(coef.data(), m->d_coef, coef.size() * sizeof(double), cudaMemcpyDeviceToHost));
-        pattern.resize((size_t)nref);
-        std::vector<uint8_t> sortkey((size_t)nref);
-        for (int64_t i = 0; i < nref; ++i) {
-            uint8_t k = 0;
-            for (int mm = 0; mm < nc1; ++mm) k |= (coef[(size_t)mm * nref + i] != 0.0) ? (uint8_t)(1u << mm) : (uint8_t)0;
-            pattern[(size_t)i] = k;
-        }
-        for (int c = 0; c < m->n_classes; ++c) {
-            // ... but only patterns that fill at least four tiles get a group of their own: splitting a small class into a dozen
-            // half-empty groups costs spatial compactness (the radius r_j of the error bound) and skips nothing
-            int count[256] = {0};
-            for (int i = start[c]; i < start[c + 1]; ++i) ++count[pattern[(size_t)i]];
-            for (int i = start[c]; i < start[c + 1]; ++i)
-                if (count[pattern[(size_t)i]] < 4 * kEN) sortkey[(size_t)i] = 255; else sortkey[(size_t)i] = pattern[(size_t)i];
-            std::stable_sort(order.begin() + start[c], order.begin() + start[c + 1],
-                             [&](int32_t a, int32_t b2) { return sortkey[(size_t)a] < sortkey[(size_t)b2]; });
-            for (size_t lo = (size_t)start[c]; lo < (size_t)start[c + 1];) {
-                size_t hi = lo + 1;
-                while (hi < (size_t)start[c + 1] && sortkey[(size_t)order[hi]] == sortkey[(size_t)order[lo]]) ++hi;
-                compact_order(ref, d, order, lo, hi);
-                lo = hi;
-            }
-            for (int r = start[c]; r < start[c + 1]; r += kEN) {
-                row0.push_back(r); rows.push_back(std::min(kEN, start[c + 1] - r)); tclass.push_back(c);
-            }
-        }
-    }
-    E->n_tiles = (int)row0.size();
-    std::vector<unsigned char> img((size_t)E->n_tiles * E->tile_bytes, 0);
-    std::vector<float> tile_tn((size_t)E->n_tiles, 0.f);
-    for (int t = 0; t < E->n_tiles; ++t) {
-        unsigned char *tile = img.data() + (size_t)t * E->tile_bytes;
-        double tc[kEMaxD], delta[kEMaxD];
-        float *hdr = nullptr;
-        double cnorm = 0.0, rmax2 = 0.0;
-        if (svc) {   // tile centre relative to c0: the mean of its rows minus c0, rounded to fp32 (the epilogue subtracts exactly this)
-            hdr = reinterpret_cast<float *>(tile + kETileB + (size_t)nc1 * kEN * sizeof(float));
-            for (int j = 0; j < d; ++j) {
-                double a = 0.0;
-                for (int r = 0; r < rows[t]; ++r) a += ref[(size_t)order[(size_t)(row0[t] + r)] * d + j];
-                const float cj = static_cast<float>(a / rows[t] - center[j]);
-                hdr[j] = cj;
-                delta[j] = (double)cj;
-                tc[j] = center[j] + (double)cj;
-                cnorm += (double)cj * (double)cj;
-            }
-            for (int j = d; j < 16; ++j) hdr[j] = 0.f;
-        }
-        for (int r = 0; r < kEN; ++r) {
-            if (r < rows[t]) {
-                const int32_t src = order[(size_t)(row0[t] + r)];
-                const double nrm = pack_row(tile, r, &ref[(size_t)src * d], svc ? tc : center.data(), svc ? delta : nullptr, d,
-                                            svc ? 1.0 : 1.0 - (double)kKappa);
-                rmax2 = std::max(rmax2, nrm);
-                if (svc) {
-                    float *cf = reinterpret_cast<float *>(tile + kETileB);
-                    for (int mm = 0; mm < nc1; ++mm) {
-                        const double cv = coef[(size_t)mm * nref + src];
-                        cf[mm * kEN + r] = static_cast<float>(cv);
-                        // libsvm's sign pattern (file header): row mm of a class-c vector faces opponent o = mm < c ? mm : mm + 1
-                        // and is >= 0 iff c < o
-                        const int o = mm < tclass[t] ? mm : mm + 1;
-                        if ((tclass[t] < o) ? (cv < 0.0) : (cv > 0.0)) E->certifiable = false;
-                    }
-                }
-            } else {
-                pack_dummy(tile, r, d, !svc);
-            }
-        }
-        tile_tn[(size_t)t] = std::nextafterf(static_cast<float>(rmax2), INFINITY);
-        if (svc) {   // constants of eta_j (file header), rounded up
-            const double rj = std::sqrt(rmax2) * (1.0 + 1e-6), cj = std::sqrt(cnorm) * (1.0 + 1e-6);
-            const double eps = (double)kSvcEpsMma, p23 = 1.0 / 8388608.0;
-            hdr[12] = std::nextafterf(static_cast<float>(m->gamma * (2.0 * eps + p23) * rj), INFINITY);
-            hdr[13] = std::nextafterf(static_cast<float>(m->gamma * eps * (rj * rj + 2.0 * cj * rj) + (double)kSvcEtaConst), INFINITY);
-            // active coefficient rows of the tile: count | row0 << 4 | row1 << 7 | ... (bit pattern stored in a float slot)
-            uint32_t mask = 0;
-            for (int r = 0; r < rows[t]; ++r) mask |= pattern[(size_t)order[(size_t)(row0[t] + r)]];
-            if (mask == 0) mask = 1;
-            uint32_t word = 0, na = 0;
-            for (int mm = 0; mm < nc1; ++mm)
-                if (mask & (1u << mm)) { word |= (uint32_t)mm << (4 + 3 * na); ++na; }
-            word |= na;
-            memcpy(&hdr[14], &word, 4);
-            hdr[15] = static_cast<float>(rj);
-        }
-    }
-    if (svc) {
-        // absolute part of E_p: rounding e = g2 d to fp32 costs K a relative ln2 2^-24 |e|; for |e| <= 4 that is inside
-        // eta_const, beyond it |e| 2^-|e| <= 1/4 bounds the ABSOLUTE error of coef K by 1.04e-8 |coef|.  Plus 1e-9 for
-        // the float accumulation of the bound itself, ex2's flush to zero and the fp64 kernel's own distance from libsvm.
-        std::vector<int32_t> start(m->n_classes + 1);
-        TCSDN_CUDA(cudaMemcpy(start.data(), m->d_start, start.size() * sizeof(int32_t), cudaMemcpyDeviceToHost));
-        const int Cn = m->n_classes;
-        int p = 0;
-        for (int i = 0; i < Cn; ++i)
-            for (int jj = i + 1; jj < Cn; ++jj, ++p) {
-                double a = 0.0;
-                for (int sidx = start[i]; sidx < start[i + 1]; ++sidx) a += std::fabs(coef[(size_t)(jj - 1) * nref + sidx]);
-                for (int sidx = start[jj]; sidx < start[jj + 1]; ++sidx) a += std::fabs(coef[(size_t)i * nref + sidx]);
-                E->eabs[p] = std::nextafterf(static_cast<float>(1.04e-8 * a + 1e-9), INFINITY);
-            }
-    }
-    int rc = upload(&E->d_tiles, img.data(), img.size());
-    if (rc == TCSDN_OK && !svc) {
-        // exact re-evaluation reads the original rows with 16-byte loads: even row stride; rows in TILE order (a candidate is
-        // (tile, column)), labels likewise
-        const int dpad = kEMaxD;
-        const size_t npos = (size_t)E->n_tiles * kEN;
-        std::vector<double> pad(npos * dpad, 0.0);
-        std::vector<int32_t> ypos(npos, 0), yh((size_t)nref), pos_orig(npos, -1);
-        TCSDN_CUDA(cudaMemcpy(yh.data(), m->d_y, yh.size() * sizeof(int32_t), cudaMemcpyDeviceToHost));
-        for (int64_t i = 0; i < nref; ++i) {
-            memcpy(&pad[(size_t)i * dpad], &ref[(size_t)order[(size_t)i] * d], (size_t)d * sizeof(double));
-            ypos[(size_t)i] = yh[(size_t)order[(size_t)i]];
-            pos_orig[(size_t)i] = order[(size_t)i];
-        }
-        rc = upload(&E->d_refpad, pad.data(), pad.size());
-        if (rc == TCSDN_OK) rc = upload(&E->d_ypos, ypos.data(), ypos.size());
-        if (rc == TCSDN_OK) rc = upload(&E->d_pos_orig, pos_orig.data(), pos_orig.size());
-        if (rc == TCSDN_OK) rc = upload(&E->d_tile_tn, tile_tn.data(), tile_tn.size());
-        // pruning tables: tile centres and radii, the kd tree, and per home tile the tiles by centre distance
-        const int nt = E->n_tiles;
-        std::vector<double> tcent((size_t)nt * d, 0.0), trad((size_t)nt, 0.0);
-        for (int t = 0; t < nt; ++t) {
-            for (int j = 0; j < d; ++j) {
-                double a = 0.0;
-                for (int r = 0; r < rows[t]; ++r) a += ref[(size_t)order[(size_t)(row0[t] + r)] * d + j];
-                tcent[(size_t)t * d + j] = a / rows[t];
-            }
-            double r2 = 0.0;
-            for (int r = 0; r < rows[t]; ++r) {
-                double a = 0.0;
-                for (int j = 0; j < d; ++j) { const double df = ref[(size_t)order[(size_t)(row0[t] + r)] * d + j] - tcent[(size_t)t * d + j]; a += df * df; }
-                r2 = std::max(r2, a);
-            }
-            trad[(size_t)t] = std::sqrt(r2) * (1.0 + 1e-9) + 1e-300;
-        }
-        if (rc == TCSDN_OK) rc = upload(&E->d_tcent, tcent.data(), tcent.size());
-        if (rc == TCSDN_OK) rc = upload(&E->d_trad, trad.data(), trad.size());
-        if (rc == TCSDN_OK) rc = upload(&E->d_kd_dim, kd.dim.data(), kd.dim.size());
-        if (rc == TCSDN_OK) rc = upload(&E->d_kd_child, kd.child.data(), kd.child.size());
-        if (rc == TCSDN_OK) rc = upload(&E->d_kd_split, kd.split.data(), kd.split.size());
-        if (rc == TCSDN_OK) rc = upload(&E->d_leaf_tile, kd.leaf_tile.data(), kd.leaf_tile.size());
-        E->n_leaves = (int)kd.leaf_tile.size();
-        if (rc == TCSDN_OK && nt <= kEMaxPruneTiles) {
-            const int nch = (nt + 31) / 32;
-            std::vector<uint16_t> nbr((size_t)nt * nt);
-            std::vector<float> clb((size_t)nt * nch);
-            std::vector<std::pair<double, int>> byd((size_t)nt);
-            for (int h = 0; h < nt; ++h) {
-                for (int t = 0; t < nt; ++t) {
-                    double a = 0.0;
-                    for (int j = 0; j < d; ++j) { const double df = tcent[(size_t)h * d + j] - tcent[(size_t)t * d + j]; a += df * df; }
-                    byd[(size_t)t] = {std::sqrt(a), t};
-                }
-                std::sort(byd.begin(), byd.end());
-                double suffix = 1e300;   // min over positions >= i of (centre distance - radius), rounded down
-                for (int i = nt - 1; i >= 0; --i) {
-                    nbr[(size_t)h * nt + i] = (uint16_t)byd[(size_t)i].second;
-                    suffix = std::min(suffix, byd[(size_t)i].first * (1.0 - 1e-9) - trad[(size_t)byd[(size_t)i].second]);
-                    if ((i & 31) == 0) clb[(size_t)h * nch + (i >> 5)] = std::nextafterf(static_cast<float>(suffix), -INFINITY);
-                }
-            }
-            rc = upload(&E->d_nbr, nbr.data(), nbr.size());
-            if (rc == TCSDN_OK) rc = upload(&E->d_chunk_lb, clb.data(), clb.size());
-        }
-        if (rc == TCSDN_OK) {   // scratch of a call: its own pool that keeps what it has allocated
-            cudaMemPoolProps props;
-            memset(&props, 0, sizeof(props));
-            props.allocType = cudaMemAllocationTypePinned;
-            props.location.type = cudaMemLocationTypeDevice;
-            props.location.id = m->dev;
-            TCSDN_CUDA(cudaMemPoolCreate(&E->pool, &props));
-            uint64_t keep = UINT64_MAX;
-            TCSDN_CUDA(cudaMemPoolSetAttribute(E->pool, cudaMemPoolAttrReleaseThreshold, &keep));
-        }
-    }
-    if (rc == TCSDN_OK) rc = upload(&E->d_tile_class, tclass.data(), tclass.size());
-    if (rc == TCSDN_OK) rc = upload(&E->d_tile_row0, row0.data(), row0.size());
-    if (rc == TCSDN_OK) rc = upload(&E->d_tile_rows, rows.data(), rows.size());
-    if (rc == TCSDN_OK) rc = upload(&E->d_center, center.data(), center.size());
-    float zero = 0.f;
-    unsigned long long zero64[32] = {};
-    if (rc == TCSDN_OK) rc = upload(&E->d_maxratio, &zero, 1);
-    if (rc == TCSDN_OK) rc = upload(&E->d_counters, zero64, 32);   // [8 ..]: experiment builds' cycle counters
-    m->engine = E;
-    if (rc != TCSDN_OK) { engine_destroy(m); return rc; }
     return TCSDN_OK;
 }
 
-void engine_destroy(tcsdn_model *m) {
-    EngineState *E = static_cast<EngineState *>(m->engine);
-    if (!E) return;
-    cudaFree(E->d_tiles); cudaFree(E->d_tile_class); cudaFree(E->d_tile_row0); cudaFree(E->d_tile_rows);
-    cudaFree(E->d_center); cudaFree(E->d_refpad); cudaFree(E->d_maxratio); cudaFree(E->d_counters);
-    cudaFree(E->d_kd_dim); cudaFree(E->d_kd_child); cudaFree(E->d_kd_split); cudaFree(E->d_leaf_tile); cudaFree(E->d_tcent); cudaFree(E->d_trad);
-    cudaFree(E->d_nbr); cudaFree(E->d_chunk_lb); cudaFree(E->d_ypos); cudaFree(E->d_tile_tn); cudaFree(E->d_pos_orig);
-    if (E->pool) cudaMemPoolDestroy(E->pool);
-    delete E;
+// Rows src[0 .. rows) of ref into the tile image (pack_row, with its `center`, `delta` and `norm_scale`), padding rows after
+// them (pack_dummy); returns the largest ||u||^2 of the packed rows
+static double pack_tile(unsigned char *tile, const std::vector<double> &ref, const int32_t *src, int rows, int d,
+                        const double *center, const double *delta, double norm_scale, bool pad_inf) {
+    double rmax2 = 0.0;
+    for (int r = 0; r < kEN; ++r) {
+        if (r < rows) rmax2 = std::max(rmax2, pack_row(tile, r, &ref[(size_t)src[r] * d], center, delta, d, norm_scale));
+        else pack_dummy(tile, r, d, pad_inf);
+    }
+    return rmax2;
+}
+
+// what both kinds upload: the tile images, the centre, the audit statistic and the counters
+static int upload_common(EngineState *E, const std::vector<unsigned char> &img, const std::vector<double> &center) {
+    const float zero = 0.f;
+    const unsigned long long zero4[4] = {};
+    TCSDN_TRY(upload(&E->d_tiles, img.data(), img.size()));
+    TCSDN_TRY(upload(&E->d_center, center.data(), center.size()));
+    TCSDN_TRY(upload(&E->d_maxratio, &zero, 1));
+    return upload(&E->d_counters, zero4, 4);
+}
+
+EngineState::~EngineState() { cudaFree(d_tiles); cudaFree(d_center); cudaFree(d_maxratio); cudaFree(d_counters); }
+
+KnnEngine::~KnnEngine() {
+    cudaFree(d_tile_rows); cudaFree(d_refpad); cudaFree(d_kd_dim); cudaFree(d_kd_child); cudaFree(d_kd_split); cudaFree(d_leaf_tile);
+    cudaFree(d_tcent); cudaFree(d_trad); cudaFree(d_nbr); cudaFree(d_chunk_lb); cudaFree(d_ypos); cudaFree(d_pos_orig); cudaFree(d_tile_tn);
+    if (pool) cudaMemPoolDestroy(pool);
+}
+
+SvcEngine::~SvcEngine() { cudaFree(d_tile_class); }
+
+int knn_engine_create(tcsdn_model *m) {
+    m->engine = nullptr;
+    const int d = m->d;
+    if (d > kEMaxD || m->k > kEMaxK) return TCSDN_OK;     // engine not applicable: fp64 kernels only
+    const int64_t nref = m->n_train;
+    std::vector<double> ref, center;
+    TCSDN_TRY(host_rows(m->d_fit, nref, d, ref, center));
+    KnnEngine *E = new KnnEngine();
+    m->engine = E;   // from here on, what an error return leaves behind is freed by engine_destroy (tcsdn_destroy)
+    E->tile_bytes = kETileB;
+    // tile plan: kd order (spatially compact tiles: whole tiles can be skipped, see the file header)
+    std::vector<int32_t> row0, rows, order((size_t)nref);
+    for (int64_t i = 0; i < nref; ++i) order[(size_t)i] = (int32_t)i;
+    KdTree kd;
+    while (kd.leaf_rows < kEN && nref / (kd.leaf_rows / 2 + 1) > kEMaxLeaves) kd.leaf_rows *= 2;   // the sort's histogram lives in shared memory
+    kd_build(ref, d, order, 0, (size_t)nref, kd);
+    for (int64_t r = 0; r < nref; r += kEN) { row0.push_back((int32_t)r); rows.push_back((int32_t)std::min<int64_t>(kEN, nref - r)); }
+    const int nt = E->n_tiles = (int)row0.size();
+    std::vector<unsigned char> img((size_t)nt * E->tile_bytes, 0);
+    std::vector<float> tile_tn((size_t)nt);
+    for (int t = 0; t < nt; ++t) {
+        const double rmax2 = pack_tile(img.data() + (size_t)t * E->tile_bytes, ref, &order[(size_t)row0[t]], rows[t], d,
+                                       center.data(), nullptr, 1.0 - (double)kKappa, true);
+        tile_tn[(size_t)t] = std::nextafterf(static_cast<float>(rmax2), INFINITY);
+    }
+    TCSDN_TRY(upload_common(E, img, center));
+    TCSDN_TRY(upload(&E->d_tile_rows, rows.data(), rows.size()));
+    // exact re-evaluation reads the original rows with 16-byte loads: even row stride; rows in TILE order (a candidate is
+    // (tile, column)), labels likewise
+    const int dpad = kEMaxD;
+    const size_t npos = (size_t)nt * kEN;
+    std::vector<double> pad(npos * dpad, 0.0);
+    std::vector<int32_t> ypos(npos, 0), yh((size_t)nref), pos_orig(npos, -1);
+    TCSDN_CUDA(cudaMemcpy(yh.data(), m->d_y, yh.size() * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    for (int64_t i = 0; i < nref; ++i) {
+        memcpy(&pad[(size_t)i * dpad], &ref[(size_t)order[(size_t)i] * d], (size_t)d * sizeof(double));
+        ypos[(size_t)i] = yh[(size_t)order[(size_t)i]];
+        pos_orig[(size_t)i] = order[(size_t)i];
+    }
+    TCSDN_TRY(upload(&E->d_refpad, pad.data(), pad.size()));
+    TCSDN_TRY(upload(&E->d_ypos, ypos.data(), ypos.size()));
+    TCSDN_TRY(upload(&E->d_pos_orig, pos_orig.data(), pos_orig.size()));
+    TCSDN_TRY(upload(&E->d_tile_tn, tile_tn.data(), tile_tn.size()));
+    // pruning tables: tile centres and radii, the kd tree, and per home tile the tiles by centre distance
+    std::vector<double> tcent((size_t)nt * d, 0.0), trad((size_t)nt, 0.0);
+    for (int t = 0; t < nt; ++t) {
+        for (int j = 0; j < d; ++j) {
+            double a = 0.0;
+            for (int r = 0; r < rows[t]; ++r) a += ref[(size_t)order[(size_t)(row0[t] + r)] * d + j];
+            tcent[(size_t)t * d + j] = a / rows[t];
+        }
+        double r2 = 0.0;
+        for (int r = 0; r < rows[t]; ++r) {
+            double a = 0.0;
+            for (int j = 0; j < d; ++j) { const double df = ref[(size_t)order[(size_t)(row0[t] + r)] * d + j] - tcent[(size_t)t * d + j]; a += df * df; }
+            r2 = std::max(r2, a);
+        }
+        trad[(size_t)t] = std::sqrt(r2) * (1.0 + 1e-9) + 1e-300;
+    }
+    TCSDN_TRY(upload(&E->d_tcent, tcent.data(), tcent.size()));
+    TCSDN_TRY(upload(&E->d_trad, trad.data(), trad.size()));
+    TCSDN_TRY(upload(&E->d_kd_dim, kd.dim.data(), kd.dim.size()));
+    TCSDN_TRY(upload(&E->d_kd_child, kd.child.data(), kd.child.size()));
+    TCSDN_TRY(upload(&E->d_kd_split, kd.split.data(), kd.split.size()));
+    TCSDN_TRY(upload(&E->d_leaf_tile, kd.leaf_tile.data(), kd.leaf_tile.size()));
+    E->n_leaves = (int)kd.leaf_tile.size();
+    if (nt <= kEMaxPruneTiles) {
+        const int nch = (nt + 31) / 32;
+        std::vector<uint16_t> nbr((size_t)nt * nt);
+        std::vector<float> clb((size_t)nt * nch);
+        std::vector<std::pair<double, int>> byd((size_t)nt);
+        for (int h = 0; h < nt; ++h) {
+            for (int t = 0; t < nt; ++t) {
+                double a = 0.0;
+                for (int j = 0; j < d; ++j) { const double df = tcent[(size_t)h * d + j] - tcent[(size_t)t * d + j]; a += df * df; }
+                byd[(size_t)t] = {std::sqrt(a), t};
+            }
+            std::sort(byd.begin(), byd.end());
+            double suffix = 1e300;   // min over positions >= i of (centre distance - radius), rounded down
+            for (int i = nt - 1; i >= 0; --i) {
+                nbr[(size_t)h * nt + i] = (uint16_t)byd[(size_t)i].second;
+                suffix = std::min(suffix, byd[(size_t)i].first * (1.0 - 1e-9) - trad[(size_t)byd[(size_t)i].second]);
+                if ((i & 31) == 0) clb[(size_t)h * nch + (i >> 5)] = std::nextafterf(static_cast<float>(suffix), -INFINITY);
+            }
+        }
+        TCSDN_TRY(upload(&E->d_nbr, nbr.data(), nbr.size()));
+        TCSDN_TRY(upload(&E->d_chunk_lb, clb.data(), clb.size()));
+    }
+    // scratch of a call: its own pool that keeps what it has allocated
+    cudaMemPoolProps props;
+    memset(&props, 0, sizeof(props));
+    props.allocType = cudaMemAllocationTypePinned;
+    props.location.type = cudaMemLocationTypeDevice;
+    props.location.id = m->dev;
+    TCSDN_CUDA(cudaMemPoolCreate(&E->pool, &props));
+    uint64_t keep = UINT64_MAX;
+    TCSDN_CUDA(cudaMemPoolSetAttribute(E->pool, cudaMemPoolAttrReleaseThreshold, &keep));
+    return TCSDN_OK;
+}
+
+int svc_engine_create(tcsdn_model *m) {
+    m->engine = nullptr;
+    const int d = m->d, nc1 = m->n_classes - 1;
+    if (d > kEMaxD || nc1 > kEMaxNC1) return TCSDN_OK;     // engine not applicable: fp64 kernels only
+    const int64_t nref = m->n_sv;
+    std::vector<double> ref, center;
+    TCSDN_TRY(host_rows(m->d_sv, nref, d, ref, center));
+    SvcEngine *E = new SvcEngine();
+    m->engine = E;   // from here on, what an error return leaves behind is freed by engine_destroy (tcsdn_destroy)
+    E->nc1 = nc1;
+    // tile image = bf16 B operand, then the tile's dual coefficients + centre
+    E->tile_bytes = kETileB + nc1 * kEN * (int)sizeof(float) + 16 * (int)sizeof(float);
+    // tile plan: per class (sums are per class), rows re-ordered inside the class for spatial compactness (sums do not
+    // care about order), padded to a tile boundary with zero-coefficient rows
+    std::vector<int32_t> row0, rows, tclass, order((size_t)nref), start(m->n_classes + 1);
+    for (int64_t i = 0; i < nref; ++i) order[(size_t)i] = (int32_t)i;
+    TCSDN_CUDA(cudaMemcpy(start.data(), m->d_start, start.size() * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    // inside a class: first by the vector's non-zero coefficient pattern (the kernel skips coefficient rows that are zero
+    // on a whole tile), then spatially compact inside every pattern group
+    std::vector<double> coef((size_t)nc1 * nref);    // dual coefficients [nc1][nref]
+    TCSDN_CUDA(cudaMemcpy(coef.data(), m->d_coef, coef.size() * sizeof(double), cudaMemcpyDeviceToHost));
+    std::vector<uint8_t> pattern((size_t)nref);      // per support vector, bit mm set iff coefficient row mm is non-zero
+    std::vector<uint8_t> sortkey((size_t)nref);
+    for (int64_t i = 0; i < nref; ++i) {
+        uint8_t k = 0;
+        for (int mm = 0; mm < nc1; ++mm) k |= (coef[(size_t)mm * nref + i] != 0.0) ? (uint8_t)(1u << mm) : (uint8_t)0;
+        pattern[(size_t)i] = k;
+    }
+    for (int c = 0; c < m->n_classes; ++c) {
+        // ... but only patterns that fill at least four tiles get a group of their own: splitting a small class into a dozen
+        // half-empty groups costs spatial compactness (the radius r_j of the error bound) and skips nothing
+        int count[256] = {0};
+        for (int i = start[c]; i < start[c + 1]; ++i) ++count[pattern[(size_t)i]];
+        for (int i = start[c]; i < start[c + 1]; ++i)
+            if (count[pattern[(size_t)i]] < 4 * kEN) sortkey[(size_t)i] = 255; else sortkey[(size_t)i] = pattern[(size_t)i];
+        std::stable_sort(order.begin() + start[c], order.begin() + start[c + 1],
+                         [&](int32_t a, int32_t b2) { return sortkey[(size_t)a] < sortkey[(size_t)b2]; });
+        for (size_t lo = (size_t)start[c]; lo < (size_t)start[c + 1];) {
+            size_t hi = lo + 1;
+            while (hi < (size_t)start[c + 1] && sortkey[(size_t)order[hi]] == sortkey[(size_t)order[lo]]) ++hi;
+            compact_order(ref, d, order, lo, hi);
+            lo = hi;
+        }
+        for (int r = start[c]; r < start[c + 1]; r += kEN) {
+            row0.push_back(r); rows.push_back(std::min(kEN, start[c + 1] - r)); tclass.push_back(c);
+        }
+    }
+    const int nt = E->n_tiles = (int)row0.size();
+    std::vector<unsigned char> img((size_t)nt * E->tile_bytes, 0);
+    for (int t = 0; t < nt; ++t) {
+        unsigned char *tile = img.data() + (size_t)t * E->tile_bytes;
+        // tile centre relative to c0: the mean of its rows minus c0, rounded to fp32 (the epilogue subtracts exactly this)
+        float *hdr = reinterpret_cast<float *>(tile + kETileB + (size_t)nc1 * kEN * sizeof(float));
+        double tc[kEMaxD], delta[kEMaxD], cnorm = 0.0;
+        for (int j = 0; j < d; ++j) {
+            double a = 0.0;
+            for (int r = 0; r < rows[t]; ++r) a += ref[(size_t)order[(size_t)(row0[t] + r)] * d + j];
+            const float cj = static_cast<float>(a / rows[t] - center[j]);
+            hdr[j] = cj;
+            delta[j] = (double)cj;
+            tc[j] = center[j] + (double)cj;
+            cnorm += (double)cj * (double)cj;
+        }
+        for (int j = d; j < 16; ++j) hdr[j] = 0.f;
+        const double rmax2 = pack_tile(tile, ref, &order[(size_t)row0[t]], rows[t], d, tc, delta, 1.0, false);
+        float *cf = reinterpret_cast<float *>(tile + kETileB);
+        for (int r = 0; r < rows[t]; ++r) {
+            const int32_t src = order[(size_t)(row0[t] + r)];
+            for (int mm = 0; mm < nc1; ++mm) {
+                const double cv = coef[(size_t)mm * nref + src];
+                cf[mm * kEN + r] = static_cast<float>(cv);
+                // libsvm's sign pattern (file header): row mm of a class-c vector faces opponent o = mm < c ? mm : mm + 1
+                // and is >= 0 iff c < o
+                const int o = mm < tclass[t] ? mm : mm + 1;
+                if ((tclass[t] < o) ? (cv < 0.0) : (cv > 0.0)) E->certifiable = false;
+            }
+        }
+        // constants of eta_j (file header), rounded up
+        const double rj = std::sqrt(rmax2) * (1.0 + 1e-6), cj = std::sqrt(cnorm) * (1.0 + 1e-6);
+        const double eps = (double)kSvcEpsMma, p23 = 1.0 / 8388608.0;
+        hdr[12] = std::nextafterf(static_cast<float>(m->gamma * (2.0 * eps + p23) * rj), INFINITY);
+        hdr[13] = std::nextafterf(static_cast<float>(m->gamma * eps * (rj * rj + 2.0 * cj * rj) + (double)kSvcEtaConst), INFINITY);
+        // active coefficient rows of the tile: count | row0 << 4 | row1 << 7 | ... (bit pattern stored in a float slot)
+        uint32_t mask = 0;
+        for (int r = 0; r < rows[t]; ++r) mask |= pattern[(size_t)order[(size_t)(row0[t] + r)]];
+        if (mask == 0) mask = 1;
+        uint32_t word = 0, na = 0;
+        for (int mm = 0; mm < nc1; ++mm)
+            if (mask & (1u << mm)) { word |= (uint32_t)mm << (4 + 3 * na); ++na; }
+        word |= na;
+        memcpy(&hdr[14], &word, 4);
+        hdr[15] = static_cast<float>(rj);
+    }
+    // absolute part of E_p: rounding e = g2 d to fp32 costs K a relative ln2 2^-24 |e|; for |e| <= 4 that is inside
+    // eta_const, beyond it |e| 2^-|e| <= 1/4 bounds the ABSOLUTE error of coef K by 1.04e-8 |coef|.  Plus 1e-9 for
+    // the float accumulation of the bound itself, ex2's flush to zero and the fp64 kernel's own distance from libsvm.
+    const int Cn = m->n_classes;
+    int p = 0;
+    for (int i = 0; i < Cn; ++i)
+        for (int jj = i + 1; jj < Cn; ++jj, ++p) {
+            double a = 0.0;
+            for (int sidx = start[i]; sidx < start[i + 1]; ++sidx) a += std::fabs(coef[(size_t)(jj - 1) * nref + sidx]);
+            for (int sidx = start[jj]; sidx < start[jj + 1]; ++sidx) a += std::fabs(coef[(size_t)i * nref + sidx]);
+            E->eabs[p] = std::nextafterf(static_cast<float>(1.04e-8 * a + 1e-9), INFINITY);
+        }
+    TCSDN_TRY(upload_common(E, img, center));
+    return upload(&E->d_tile_class, tclass.data(), tclass.size());
+}
+
+void engine_destroy(tcsdn_model *m) {   // m->engine holds the engine of the handle's kind
+    if (m->kind == TCSDN_KIND_SVC) delete static_cast<SvcEngine *>(m->engine);
+    else delete static_cast<KnnEngine *>(m->engine);
     m->engine = nullptr;
 }
 
 bool engine_usable(const tcsdn_model *m, int64_t n, bool want_scores) {
-    const EngineState *E = static_cast<const EngineState *>(m->engine);
-    if (!E) return false;
+    if (!m->engine) return false;
     if (m->kind == TCSDN_KIND_SVC) {
-        if (!E->certifiable) return false;                     // the certificate needs libsvm's coefficient signs
+        if (!static_cast<const SvcEngine *>(m->engine)->certifiable) return false;   // the certificate needs libsvm's coefficient signs
         if (want_scores != (m->opt_engine >= 3)) return false; // decision values: fp64 kernel; audit modes fill scores
     } else if (m->opt_engine == 4) return false;
     if (m->opt_engine >= 2) return true;
     return n >= 4096;   // below this the fp64 CUDA-core kernels (latency path) are faster than filling every SM with 256-row passes
 }
 
-// kk: neighbours kept per query (KNN: the model's k for predict, the call's n_neighbors for kneighbors); nb_ind non-null
-// selects the kneighbors instantiations, which write nb_ind / nb_dist instead of labels / scores
-template <typename T>
-static int launch_engine_t(tcsdn_model *m, const T *x, int64_t n, int32_t *labels, double *scores, int32_t *flag,
-                           cudaStream_t st, int kk, int64_t *nb_ind, double *nb_dist) {
-    EngineState *E = static_cast<EngineState *>(m->engine);
-    const bool svc = m->kind == TCSDN_KIND_SVC;
-    EngineArgs A;
-    A.tiles = E->d_tiles; A.tile_class = E->d_tile_class; A.tile_row0 = E->d_tile_row0;
-    A.tile_rows = E->d_tile_rows; A.center = E->d_center; A.ref = m->d_fit; A.y = m->d_y; A.rho = m->d_rho;
+// the arguments both kernels take
+static void common_args(EngineArgs &A, const tcsdn_model *m, const EngineState *E, int64_t n, int32_t *flag) {
+    A.tiles = E->d_tiles; A.center = E->d_center;
     // audit mode (engine option 3): KNN -- the filter is disabled so that EVERY pair is re-evaluated exactly; both -- the
     // largest |tensor-core value - exact| / (error model's denominator) is recorded (stats[5]); tests only
     A.maxratio = m->opt_engine == 3 ? E->d_maxratio : nullptr;
-    A.flag = flag; A.n = n; A.n_tiles = E->n_tiles;
-    A.tile_bytes = E->tile_bytes; A.d = m->d; A.k = kk; A.C = m->n_classes; A.nc1 = E->nc1;
+    A.flag = flag; A.n = n; A.n_tiles = E->n_tiles; A.tile_bytes = E->tile_bytes; A.d = m->d;
+}
+
+static unsigned engine_grid(const tcsdn_model *m, int64_t n) {   // persistent: at most one CTA per SM
+    return (unsigned)std::min<int64_t>((n + kERows - 1) / kERows, (int64_t)m->sm_count);
+}
+
+template <typename T, bool AUDIT, KnnOut OUT>
+static auto knn_kernel(bool heap_smem) {
+    return heap_smem ? knn_engine_kernel<T, true, AUDIT, OUT> : knn_engine_kernel<T, false, AUDIT, OUT>;
+}
+
+// kk: neighbours kept per query (the model's k for predict, the call's n_neighbors for kneighbors); KnnOut::Neighbors writes
+// nb_ind / nb_dist instead of labels / scores
+template <typename T>
+static int knn_engine_run(tcsdn_model *m, const T *x, int64_t n, int32_t *labels, double *scores, int32_t *flag,
+                          cudaStream_t st, KnnOut out, int kk, int64_t *nb_ind, double *nb_dist) {
+    KnnEngine *E = static_cast<KnnEngine *>(m->engine);
+    KnnArgs A;
+    common_args(A, m, E, n, flag);
+    A.tile_rows = E->d_tile_rows; A.y = m->d_y; A.k = kk; A.C = m->n_classes;
     A.pos_orig = E->d_pos_orig; A.nb_ind = nb_ind; A.nb_dist = nb_dist;
     A.refpad = E->d_refpad; A.dpad = kEMaxD;
     A.flush_tiles = m->opt_knn_flush > 0 ? (int)m->opt_knn_flush : kEFlushTiles;   // TCSDN_OPT_KNN_FLUSH_TILES
-    A.n_ref = (int)(svc ? m->n_sv : m->n_train);
-    A.g2 = static_cast<float>(-m->gamma * 1.4426950408889634);
-    A.svc_mode = svc && m->opt_engine >= 3 ? (int)m->opt_engine : 0;
-    A.svc_c1 = std::nextafterf(static_cast<float>(m->gamma * (1.0 / 1048576.0 + 1.0 / 16777216.0)), INFINITY);
-    A.svc_c2 = std::nextafterf(static_cast<float>(m->gamma / 16777216.0), INFINITY);
-    for (int p = 0; p < (kEMaxNC1 + 1) * kEMaxNC1 / 2; ++p) A.svc_eabs[p] = E->eabs[p];
-    const bool heap_smem = !svc && kk <= kEHeapSmemK;
-    const int P = m->n_classes * (m->n_classes - 1) / 2;
-    // KNN: order the queries by home tile (counting sort on this stream) so that a pass's 256 rows are neighbours and the
+    const bool heap_smem = kk <= kEHeapSmemK;
+    // Order the queries by home tile (counting sort on this stream) so that a pass's 256 rows are neighbours and the
     // producer can leave out the tiles that are too far for all of them.  Scratch comes from the engine's own stream-ordered
     // pool (capturable into a CUDA graph, private to the call).
     A.ypos = E->d_ypos; A.tcent = E->d_tcent; A.trad = E->d_trad; A.chunk_lb = E->d_chunk_lb; A.tile_tn = E->d_tile_tn;
-    A.nbr = nullptr; A.qperm = nullptr; A.qkey = nullptr; A.leaf_tile = nullptr; A.tie_list = nullptr; A.tie_count = nullptr;
+    A.nbr = nullptr; A.qperm = nullptr; A.qkey = nullptr; A.leaf_tile = nullptr;
     struct ScratchGuard {   // the call's scratch goes back to the pool behind everything enqueued so far, on every return path
         int32_t *p = nullptr;
         cudaStream_t st = nullptr;
         ~ScratchGuard() { if (p) cudaFreeAsync(p, st); }
     } scratch_guard;
     int32_t *scratch = nullptr;
-    if (!svc) {
-        const int n_blocks = 2 * m->sm_count, n_bins = E->n_leaves;
-        const size_t hsm = (size_t)n_bins * sizeof(int32_t);   // the sort's histogram: shared memory
-        const bool prune = m->opt_knn_prune != 1 && A.maxratio == nullptr && n < ((int64_t)1 << 31) && hsm <= 200 * 1024;
-        const size_t n_al = ((size_t)n + 3) & ~(size_t)3;
-        // layout (int32): tie_count[4] | tie_list[n] | key[n] | perm[n] | bin_start[bins] | block_hist[blocks][bins]
-        const size_t words = 4 + n_al + (prune ? 2 * n_al + (size_t)n_bins + (size_t)n_blocks * n_bins : 0);
-        TCSDN_CUDA(cudaMallocFromPoolAsync(reinterpret_cast<void **>(&scratch), words * sizeof(int32_t), E->pool, st));
-        scratch_guard.p = scratch;
-        scratch_guard.st = st;
-        TCSDN_CUDA(cudaMemsetAsync(scratch, 0, 4 * sizeof(int32_t), st));
-        A.tie_count = scratch;
-        A.tie_list = scratch + 4;
-        if (prune) {
-            int32_t *key = scratch + 4 + n_al, *perm = key + n_al, *bin_start = perm + n_al, *block_hist = bin_start + n_bins;
-            const int64_t rpb = (n + n_blocks - 1) / n_blocks;
-            if (hsm > 48 * 1024) {
-                TCSDN_CUDA(cudaFuncSetAttribute(knn_key_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hsm));
-                TCSDN_CUDA(cudaFuncSetAttribute(knn_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hsm));
-                TCSDN_CUDA(cudaFuncSetAttribute(knn_scatter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hsm));
-            }
-            knn_key_kernel<T><<<n_blocks, kSortThreads, hsm, st>>>(x, n, m->d, rpb, E->d_kd_dim, E->d_kd_child, E->d_kd_split, n_bins, key, block_hist);
-            knn_scan_kernel<<<1, 1024, hsm, st>>>(block_hist, n_blocks, n_bins, bin_start);
-            knn_scatter_kernel<<<n_blocks, kSortThreads, hsm, st>>>(key, n, rpb, block_hist, bin_start, n_bins, perm);
-            TCSDN_CUDA(cudaGetLastError());
-            m->stats[0] += 3;
-            A.nbr = E->d_nbr;   // nullptr beyond kEMaxPruneTiles: the producer walks outwards in kd order instead
-            A.qperm = perm; A.qkey = key; A.leaf_tile = E->d_leaf_tile;
+    const int n_blocks = 2 * m->sm_count, n_bins = E->n_leaves;
+    const size_t hsm = (size_t)n_bins * sizeof(int32_t);   // the sort's histogram: shared memory
+    const bool prune = m->opt_knn_prune != 1 && A.maxratio == nullptr && n < ((int64_t)1 << 31) && hsm <= 200 * 1024;
+    const size_t n_al = ((size_t)n + 3) & ~(size_t)3;
+    // layout (int32): tie_count[4] | tie_list[n] | key[n] | perm[n] | bin_start[bins] | block_hist[blocks][bins]
+    const size_t words = 4 + n_al + (prune ? 2 * n_al + (size_t)n_bins + (size_t)n_blocks * n_bins : 0);
+    TCSDN_CUDA(cudaMallocFromPoolAsync(reinterpret_cast<void **>(&scratch), words * sizeof(int32_t), E->pool, st));
+    scratch_guard.p = scratch;
+    scratch_guard.st = st;
+    TCSDN_CUDA(cudaMemsetAsync(scratch, 0, 4 * sizeof(int32_t), st));
+    A.tie_count = scratch;
+    A.tie_list = scratch + 4;
+    if (prune) {
+        int32_t *key = scratch + 4 + n_al, *perm = key + n_al, *bin_start = perm + n_al, *block_hist = bin_start + n_bins;
+        const int64_t rpb = (n + n_blocks - 1) / n_blocks;
+        if (hsm > 48 * 1024) {
+            TCSDN_CUDA(cudaFuncSetAttribute(knn_key_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hsm));
+            TCSDN_CUDA(cudaFuncSetAttribute(knn_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hsm));
+            TCSDN_CUDA(cudaFuncSetAttribute(knn_scatter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hsm));
         }
+        knn_key_kernel<T><<<n_blocks, kSortThreads, hsm, st>>>(x, n, m->d, rpb, E->d_kd_dim, E->d_kd_child, E->d_kd_split, n_bins, key, block_hist);
+        knn_scan_kernel<<<1, 1024, hsm, st>>>(block_hist, n_blocks, n_bins, bin_start);
+        knn_scatter_kernel<<<n_blocks, kSortThreads, hsm, st>>>(key, n, rpb, block_hist, bin_start, n_bins, perm);
+        TCSDN_CUDA(cudaGetLastError());
+        m->stats[0] += 3;
+        A.nbr = E->d_nbr;   // nullptr beyond kEMaxPruneTiles: the producer walks outwards in kd order instead
+        A.qperm = perm; A.qkey = key; A.leaf_tile = E->d_leaf_tile;
     }
-    const int rows_per_pass = svc ? kERows : kKnnRows;
-    const size_t smem = (size_t)(rows_per_pass / 128) * kEATile + kETBytes + (size_t)kEStages * E->tile_bytes + kEBarRegion +
-                        (svc ? (size_t)P * kERows * (sizeof(double) + sizeof(float))
-                             : kKnnRows * (size_t)kEListCap * sizeof(uint16_t) + (heap_smem ? kKnnRows * (size_t)kk * 12 : 0));
-    const int64_t n_super = (n + rows_per_pass - 1) / rows_per_pass;
-    const unsigned grid = (unsigned)std::min<int64_t>(n_super, (int64_t)m->sm_count);
-#define TCSDN_LAUNCH(SVCF, NC)                                                                                    \
-    {                                                                                                             \
-        auto kern = (SVCF && A.maxratio) ? engine_kernel<T, SVCF, NC, SVCF> : engine_kernel<T, SVCF, NC, false>;   \
-        TCSDN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));           \
-        kern<<<grid, SVCF ? kESvcThreads : kEKnnThreads, smem, st>>>(A, x, labels, scores, E->d_counters);        \
+    const size_t smem = e_smem_bytes(E->tile_bytes) + kERows * (size_t)kEListCap * sizeof(uint16_t) +
+                        (heap_smem ? kERows * (size_t)kk * 12 : 0);
+    decltype(&knn_engine_kernel<T, false, false, KnnOut::Vote>) kern;
+    if (A.maxratio) {
+        if (out != KnnOut::Vote) { set_error("knn engine: kneighbors and distance weights have no audit mode"); return TCSDN_EINVAL; }
+        kern = knn_kernel<T, true, KnnOut::Vote>(heap_smem);
+    } else if (out == KnnOut::Vote) {
+        kern = knn_kernel<T, false, KnnOut::Vote>(heap_smem);
+    } else if (out == KnnOut::WeightedVote) {
+        kern = knn_kernel<T, false, KnnOut::WeightedVote>(heap_smem);
+    } else {
+        kern = knn_kernel<T, false, KnnOut::Neighbors>(heap_smem);
     }
-    if (!svc) {
-        // the distance-weighted vote (bit 3) belongs to predict on weights='distance' handles; kneighbors has no vote
-        const bool wd = !nb_ind && m->knn_weights == TCSDN_KNN_DISTANCE;
-        const int variant = (heap_smem ? 1 : 0) | (A.maxratio ? 2 : 0) | (nb_ind ? 4 : 0) | (wd ? 8 : 0);
-        switch (variant) {
-            case 0: TCSDN_LAUNCH(false, 0) break;
-            case 1: TCSDN_LAUNCH(false, 1) break;
-            case 2: TCSDN_LAUNCH(false, 2) break;
-            case 3: TCSDN_LAUNCH(false, 3) break;
-            case 4: TCSDN_LAUNCH(false, 4) break;
-            case 5: TCSDN_LAUNCH(false, 5) break;
-            case 8: TCSDN_LAUNCH(false, 8) break;
-            case 9: TCSDN_LAUNCH(false, 9) break;
-            default: set_error("knn engine: kneighbors and distance weights have no audit mode"); return TCSDN_EINVAL;
-        }
-    }
-    else switch (E->nc1) {
-        case 1: TCSDN_LAUNCH(true, 1) break;
-        case 2: TCSDN_LAUNCH(true, 2) break;
-        case 3: TCSDN_LAUNCH(true, 3) break;
-        case 4: TCSDN_LAUNCH(true, 4) break;
-        case 5: TCSDN_LAUNCH(true, 5) break;
-        default: set_error("svc engine: unsupported class count"); return TCSDN_EINVAL;
-    }
-#undef TCSDN_LAUNCH
+    TCSDN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kern<<<engine_grid(m, n), kEKnnThreads, smem, st>>>(A, x, labels, scores, E->d_counters);
     TCSDN_CUDA(cudaGetLastError());
     m->stats[0] += 1;
     m->stats[1] += n;
-    // SVC: rows the certificate could not decide carry -1 - label; the fp64 kernel re-evaluates exactly those (same stream)
-    if (svc && A.svc_mode == 0) return launch_svc_marked(m, x, n, sizeof(T) == 4 ? TCSDN_F32 : TCSDN_F64, labels, E->d_counters, st);
-    if (!svc && nb_ind)   // kneighbors: rows whose neighbour SET hangs on a tie at the k-th distance, likewise
-        return launch_knn_marked_kneighbors(m, x, n, sizeof(T) == 4 ? TCSDN_F32 : TCSDN_F64, kk, nb_ind, nb_dist, A.tie_list,
-                                            A.tie_count, E->d_counters + 1, st);
-    if (!svc) {   // KNN: rows whose label hangs on a tie at the k-th distance get sklearn's index-order heap (knn.cu)
-        return launch_knn_marked(m, x, n, sizeof(T) == 4 ? TCSDN_F32 : TCSDN_F64, labels, scores, A.tie_list, A.tie_count,
-                                 E->d_counters + 1, st);
+    // rows whose result hangs on a tie at the k-th distance get sklearn's index-order heap (knn.cu), on the same stream
+    const int dtype = sizeof(T) == 4 ? TCSDN_F32 : TCSDN_F64;
+    if (out == KnnOut::Neighbors)
+        return launch_knn_marked_kneighbors(m, x, n, dtype, kk, nb_ind, nb_dist, A.tie_list, A.tie_count, E->d_counters + 1, st);
+    return launch_knn_marked(m, x, n, dtype, labels, scores, A.tie_list, A.tie_count, E->d_counters + 1, st);
+}
+
+template <typename T, int NC1>
+static auto svc_kernel(bool audit) {
+    return audit ? svc_engine_kernel<T, NC1, true> : svc_engine_kernel<T, NC1, false>;
+}
+
+template <typename T>
+static int svc_engine_run(tcsdn_model *m, const T *x, int64_t n, int32_t *labels, double *scores, int32_t *flag,
+                          cudaStream_t st) {
+    SvcEngine *E = static_cast<SvcEngine *>(m->engine);
+    SvcArgs A;
+    common_args(A, m, E, n, flag);
+    A.tile_class = E->d_tile_class; A.rho = m->d_rho;
+    A.g2 = static_cast<float>(-m->gamma * 1.4426950408889634);
+    A.svc_mode = m->opt_engine >= 3 ? (int)m->opt_engine : 0;
+    A.svc_c1 = std::nextafterf(static_cast<float>(m->gamma * (1.0 / 1048576.0 + 1.0 / 16777216.0)), INFINITY);
+    A.svc_c2 = std::nextafterf(static_cast<float>(m->gamma / 16777216.0), INFINITY);
+    for (int p = 0; p < (kEMaxNC1 + 1) * kEMaxNC1 / 2; ++p) A.svc_eabs[p] = E->eabs[p];
+    const int P = m->n_classes * (m->n_classes - 1) / 2;
+    const size_t smem = e_smem_bytes(E->tile_bytes) + (size_t)P * kERows * (sizeof(double) + sizeof(float));
+    const bool audit = A.maxratio != nullptr;
+    decltype(&svc_engine_kernel<T, 1, false>) kern;
+    switch (E->nc1) {
+        case 1: kern = svc_kernel<T, 1>(audit); break;
+        case 2: kern = svc_kernel<T, 2>(audit); break;
+        case 3: kern = svc_kernel<T, 3>(audit); break;
+        case 4: kern = svc_kernel<T, 4>(audit); break;
+        case 5: kern = svc_kernel<T, 5>(audit); break;
+        default: set_error("svc engine: unsupported class count"); return TCSDN_EINVAL;
     }
+    TCSDN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kern<<<engine_grid(m, n), kESvcThreads, smem, st>>>(A, x, labels, scores);
+    TCSDN_CUDA(cudaGetLastError());
+    m->stats[0] += 1;
+    m->stats[1] += n;
+    // rows the certificate could not decide carry -1 - label; the fp64 kernel re-evaluates exactly those (same stream)
+    if (A.svc_mode == 0) return launch_svc_marked(m, x, n, sizeof(T) == 4 ? TCSDN_F32 : TCSDN_F64, labels, E->d_counters, st);
     return TCSDN_OK;
 }
 
-int launch_engine(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, double *scores, int32_t *flag,
-                  cudaStream_t st) {
+int launch_knn_engine(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, double *scores, int32_t *flag,
+                      cudaStream_t st) {
     if (n == 0) return TCSDN_OK;
-    if (dtype == TCSDN_F32) return launch_engine_t<float>(m, static_cast<const float *>(x), n, labels, scores, flag, st, m->k, nullptr, nullptr);
-    return launch_engine_t<double>(m, static_cast<const double *>(x), n, labels, scores, flag, st, m->k, nullptr, nullptr);
+    // the distance-weighted vote belongs to predict on weights='distance' handles
+    const KnnOut out = m->knn_weights == TCSDN_KNN_DISTANCE ? KnnOut::WeightedVote : KnnOut::Vote;
+    if (dtype == TCSDN_F32) return knn_engine_run<float>(m, static_cast<const float *>(x), n, labels, scores, flag, st, out, m->k, nullptr, nullptr);
+    return knn_engine_run<double>(m, static_cast<const double *>(x), n, labels, scores, flag, st, out, m->k, nullptr, nullptr);
 }
 
 bool engine_kneighbors_usable(const tcsdn_model *m, int64_t n, int nn) {
     return m->kind == TCSDN_KIND_KNN && nn <= kEMaxK && engine_usable(m, n, false);
 }
 
-int launch_engine_kneighbors(tcsdn_model *m, const void *x, int64_t n, int dtype, int nn, int64_t *ind, double *dist,
-                             int32_t *flag, cudaStream_t st) {
+int launch_knn_engine_kneighbors(tcsdn_model *m, const void *x, int64_t n, int dtype, int nn, int64_t *ind, double *dist,
+                                 int32_t *flag, cudaStream_t st) {
     if (n == 0) return TCSDN_OK;
-    if (dtype == TCSDN_F32) return launch_engine_t<float>(m, static_cast<const float *>(x), n, nullptr, nullptr, flag, st, nn, ind, dist);
-    return launch_engine_t<double>(m, static_cast<const double *>(x), n, nullptr, nullptr, flag, st, nn, ind, dist);
+    if (dtype == TCSDN_F32)
+        return knn_engine_run<float>(m, static_cast<const float *>(x), n, nullptr, nullptr, flag, st, KnnOut::Neighbors, nn, ind, dist);
+    return knn_engine_run<double>(m, static_cast<const double *>(x), n, nullptr, nullptr, flag, st, KnnOut::Neighbors, nn, ind, dist);
+}
+
+int launch_svc_engine(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, double *scores, int32_t *flag,
+                      cudaStream_t st) {
+    if (n == 0) return TCSDN_OK;
+    if (dtype == TCSDN_F32) return svc_engine_run<float>(m, static_cast<const float *>(x), n, labels, scores, flag, st);
+    return svc_engine_run<double>(m, static_cast<const double *>(x), n, labels, scores, flag, st);
 }
 
 // cumulative engine counters since create() (synchronising read): out[3] exact re-evaluations of the knn filter,
 // out[5] largest audited error ratio * 2^40, out[6] svc rows handed to the fp64 kernel
 void engine_read_stats(const tcsdn_model *m, int64_t *out) {
-    EngineState *E = static_cast<EngineState *>(m->engine);
-    if (!E) return;
+    if (!m->engine) return;
+    const EngineState *E = m->kind == TCSDN_KIND_SVC ? static_cast<const EngineState *>(static_cast<const SvcEngine *>(m->engine))
+                                                     : static_cast<const KnnEngine *>(m->engine);
     unsigned long long c = 0;
     float v = 0.f;
     unsigned long long c4[4] = {0, 0, 0, 0};
@@ -1807,18 +1854,6 @@ void engine_read_stats(const tcsdn_model *m, int64_t *out) {
         }
     }
     if (cudaMemcpy(&v, E->d_maxratio, sizeof(v), cudaMemcpyDeviceToHost) == cudaSuccess) out[5] = (int64_t)((double)v * 1099511627776.0);
-#if defined(TCSDN_EXP_KNN_TIMING)
-    unsigned long long kt[32];
-    if (cudaMemcpy(kt, E->d_counters, sizeof(kt), cudaMemcpyDeviceToHost) == cudaSuccess) {
-        static const char *names[3] = {"producer (lane 0): aFull wait, pass setup, chunk gaps, emptyB wait", "(unused)",
-                                       "epilogue (8 lane-0s): pack, rounds, fullB wait, skipped tiles, filtered tiles, votes"};
-        for (int r = 0; r < 3; ++r) {
-            fprintf(stderr, "KT %s:", names[r]);
-            for (int i = 0; i < 8; ++i) fprintf(stderr, " %.3e", (double)kt[8 + r * 8 + i]);
-            fprintf(stderr, "\n");
-        }
-    }
-#endif
 }
 
 }  // namespace tcsdn

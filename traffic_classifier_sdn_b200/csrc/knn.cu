@@ -10,9 +10,9 @@
 // for small batches (the reference's own call is one row at a time, traffic_classifier.py:106), as the
 // engine's exact re-evaluation rule, and as the engine's cross-check in the tests.  One thread owns one
 // query and scans the training rows in index order out of a shared-memory tile (all lanes read the same
-// training row: broadcast), so the heap sees exactly sklearn's push sequence.  Both kernels have a kneighbors mode (template
-// flag KNB): the same heap, then the kept rows in ascending (distance, index) order instead of the vote; and a distance-weighted
-// vote (template flag WD, weights='distance'): the same heap, then knn_weighted_vote (common.h) instead of the count.
+// training row: broadcast), so the heap sees exactly sklearn's push sequence.  Both kernels take the output as a template
+// parameter (KnnOut, common.h): the vote, the distance-weighted vote (weights='distance') or, for kneighbors, the kept rows in
+// ascending (distance, index) order -- the same heap, then knn_finish.
 #include <cfloat>
 
 #include "common.h"
@@ -22,6 +22,11 @@ namespace tcsdn {
 constexpr int kKnnThreads = 128;
 constexpr int kKnnTile = 128;    // training rows per shared-memory tile
 constexpr int kKnnMaxK = 64;
+
+// the distance-weighted vote is a predict mode of weights='distance' handles; kneighbors has no vote
+static KnnOut predict_out(const tcsdn_model *m) {
+    return m->knn_weights == TCSDN_KNN_DISTANCE ? KnnOut::WeightedVote : KnnOut::Vote;
+}
 
 __device__ __forceinline__ void heap_push_dev(double *values, int32_t *indices, int size, double val, int32_t val_idx) {
     // caller has already checked val < values[0]
@@ -46,10 +51,9 @@ __device__ __forceinline__ void heap_push_dev(double *values, int32_t *indices, 
     indices[cur] = val_idx;
 }
 
-// KNB (kneighbors): instead of the vote, the k kept rows in ascending (distance, index) order go to nb_ind / nb_dist
-// [n][k] (nb_dist nullable); labels and proba are unused.  The predict instantiation ignores the two trailing arguments.
-// WD (weights='distance'): label and proba from the distance-weighted vote.
-template <typename T, bool KNB = false, bool WD = false>
+// OUT == KnnOut::Neighbors (kneighbors) writes nb_ind / nb_dist [n][k] (nb_dist nullable) and leaves labels and proba
+// unused; the votes ignore the two trailing arguments.
+template <typename T, KnnOut OUT>
 __global__ void __launch_bounds__(kKnnThreads) knn_exact_kernel(const T *__restrict__ X, int64_t n, int d,
                                                                 const double *__restrict__ fit,
                                                                 const int32_t *__restrict__ y, int64_t n_train,
@@ -91,27 +95,20 @@ __global__ void __launch_bounds__(kKnnThreads) knn_exact_kernel(const T *__restr
                 }
             }
         }
-        if constexpr (KNB) {
-            if (live) knn_write_neighbors<1>(hv, hi, k, nb_ind + q * k, nb_dist ? nb_dist + q * k : nullptr);
-        } else if constexpr (WD) {
-            if (live) knn_weighted_vote<1>(hv, hi, k, C, y, labels + q, proba ? proba + q * C : nullptr);
-        } else if (live) {
-            int best = 0, arg = 0;
-            for (int c = 0; c < C; ++c) {
-                int cnt = 0;
-                for (int s = 0; s < k; ++s) cnt += (y[hi[s]] == c);
-                if (proba) proba[q * C + c] = (double)cnt / (double)k;
-                if (cnt > best) { best = cnt; arg = c; }
-            }
-            labels[q] = arg;
-        }
+        if (live) knn_finish<OUT, 1>(hv, hi, k, C, y, q, labels, proba, nb_ind, nb_dist);
     }
     if (flag && nf != nf) atomicOr(flag, 1);
 }
 
-// predict (nb_ind == nullptr: labels / scores, the model's k) or kneighbors (nb_ind / nb_dist, k = the call's n_neighbors)
-template <bool KNB>
-static int launch_exact(tcsdn_model *m, const void *x, int64_t n, int dtype, int k, int32_t *labels, double *scores,
+template <typename T>
+static auto exact_kernel(KnnOut out) {
+    return out == KnnOut::Neighbors      ? knn_exact_kernel<T, KnnOut::Neighbors>
+           : out == KnnOut::WeightedVote ? knn_exact_kernel<T, KnnOut::WeightedVote>
+                                         : knn_exact_kernel<T, KnnOut::Vote>;
+}
+
+// predict (labels / scores, the model's k) or kneighbors (nb_ind / nb_dist, k = the call's n_neighbors)
+static int launch_exact(tcsdn_model *m, const void *x, int64_t n, int dtype, KnnOut out, int k, int32_t *labels, double *scores,
                         int64_t *nb_ind, double *nb_dist, int32_t *flag, cudaStream_t st) {
     if (n == 0) return TCSDN_OK;
     const size_t smem = ((size_t)m->d * kKnnThreads + (size_t)kKnnTile * m->d) * sizeof(double);
@@ -120,15 +117,13 @@ static int launch_exact(tcsdn_model *m, const void *x, int64_t n, int dtype, int
     if (blocks > cap) blocks = cap;
     m->stats[0] += 1;
     m->stats[2] += n;
-    // the distance-weighted vote is a predict mode of weights='distance' handles; kneighbors has no vote
-    const bool wd = !KNB && m->knn_weights == TCSDN_KNN_DISTANCE;
     if (dtype == TCSDN_F32) {
-        auto kern = wd ? knn_exact_kernel<float, KNB, !KNB> : knn_exact_kernel<float, KNB, false>;
+        auto kern = exact_kernel<float>(out);
         TCSDN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kern<<<(unsigned)blocks, kKnnThreads, smem, st>>>(static_cast<const float *>(x), n, m->d, m->d_fit, m->d_y,
                                                           m->n_train, k, m->n_classes, labels, scores, flag, nb_ind, nb_dist);
     } else {
-        auto kern = wd ? knn_exact_kernel<double, KNB, !KNB> : knn_exact_kernel<double, KNB, false>;
+        auto kern = exact_kernel<double>(out);
         TCSDN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kern<<<(unsigned)blocks, kKnnThreads, smem, st>>>(static_cast<const double *>(x), n, m->d, m->d_fit, m->d_y,
                                                           m->n_train, k, m->n_classes, labels, scores, flag, nb_ind, nb_dist);
@@ -139,12 +134,12 @@ static int launch_exact(tcsdn_model *m, const void *x, int64_t n, int dtype, int
 
 int launch_knn_exact(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, double *scores,
                      int32_t *flag, cudaStream_t st) {
-    return launch_exact<false>(m, x, n, dtype, m->k, labels, scores, nullptr, nullptr, flag, st);
+    return launch_exact(m, x, n, dtype, predict_out(m), m->k, labels, scores, nullptr, nullptr, flag, st);
 }
 
 int launch_knn_exact_kneighbors(tcsdn_model *m, const void *x, int64_t n, int dtype, int nn, int64_t *ind, double *dist,
                                 int32_t *flag, cudaStream_t st) {
-    return launch_exact<true>(m, x, n, dtype, nn, nullptr, nullptr, ind, dist, flag, st);
+    return launch_exact(m, x, n, dtype, KnnOut::Neighbors, nn, nullptr, nullptr, ind, dist, flag, st);
 }
 
 // The tensor-core engine's tie rows (dist_engine.cu): a few rows per ten thousand whose label depends on which of several
@@ -153,9 +148,8 @@ int launch_knn_exact_kneighbors(tcsdn_model *m, const void *x, int64_t n, int dt
 // in step -- the sequential heap's result at 1/32 of its latency.  The number of rows is only known on the device.
 constexpr int kTieMaxD = 12;   // the engine's feature limit
 
-// KNB (kneighbors): lane 0 writes the k kept rows in ascending (distance, index) order to nb_ind / nb_dist instead of the vote;
-// WD (weights='distance'): lane 0 casts the distance-weighted vote
-template <typename T, bool KNB = false, bool WD = false>
+// lane 0 finishes the row (knn_finish)
+template <typename T, KnnOut OUT>
 __global__ void __launch_bounds__(256) knn_tie_kernel(const T *__restrict__ X, int d, const double *__restrict__ fit,
                                                       const int32_t *__restrict__ y, int64_t n_train, int k, int C,
                                                       int32_t *__restrict__ labels, double *__restrict__ proba,
@@ -205,25 +199,18 @@ __global__ void __launch_bounds__(256) knn_tie_kernel(const T *__restrict__ X, i
                 }
             }
         }
-        if constexpr (KNB) {
-            if (lane == 0) knn_write_neighbors<1>(hv, hi, k, nb_ind + q * k, nb_dist ? nb_dist + q * k : nullptr);
-        } else if constexpr (WD) {
-            if (lane == 0) knn_weighted_vote<1>(hv, hi, k, C, y, labels + q, proba ? proba + q * C : nullptr);
-        } else if (lane == 0) {
-            int best = 0, arg = 0;
-            for (int c = 0; c < C; ++c) {
-                int cnt = 0;
-                for (int s = 0; s < k; ++s) cnt += (y[hi[s]] == c);
-                if (proba) proba[q * C + c] = (double)cnt / (double)k;
-                if (cnt > best) { best = cnt; arg = c; }
-            }
-            labels[q] = arg;
-        }
+        if (lane == 0) knn_finish<OUT, 1>(hv, hi, k, C, y, q, labels, proba, nb_ind, nb_dist);
     }
 }
 
-template <bool KNB>
-static int launch_marked(tcsdn_model *m, const void *x, int64_t n, int dtype, int k, int32_t *labels, double *scores,
+template <typename T>
+static auto tie_kernel(KnnOut out) {
+    return out == KnnOut::Neighbors      ? knn_tie_kernel<T, KnnOut::Neighbors>
+           : out == KnnOut::WeightedVote ? knn_tie_kernel<T, KnnOut::WeightedVote>
+                                         : knn_tie_kernel<T, KnnOut::Vote>;
+}
+
+static int launch_marked(tcsdn_model *m, const void *x, int64_t n, int dtype, KnnOut out, int k, int32_t *labels, double *scores,
                          int64_t *nb_ind, double *nb_dist, const int32_t *list, const int *count, unsigned long long *total,
                          cudaStream_t st) {
     if (n == 0) return TCSDN_OK;
@@ -232,13 +219,12 @@ static int launch_marked(tcsdn_model *m, const void *x, int64_t n, int dtype, in
     const int64_t cap = (int64_t)m->sm_count * 4;
     if (blocks > cap) blocks = cap;
     m->stats[0] += 1;
-    const bool wd = !KNB && m->knn_weights == TCSDN_KNN_DISTANCE;
     if (dtype == TCSDN_F32) {
-        auto kern = wd ? knn_tie_kernel<float, KNB, !KNB> : knn_tie_kernel<float, KNB, false>;
+        auto kern = tie_kernel<float>(out);
         kern<<<(unsigned)blocks, 256, 0, st>>>(static_cast<const float *>(x), m->d, m->d_fit, m->d_y, m->n_train, k, m->n_classes,
                                                labels, scores, list, count, total, nb_ind, nb_dist);
     } else {
-        auto kern = wd ? knn_tie_kernel<double, KNB, !KNB> : knn_tie_kernel<double, KNB, false>;
+        auto kern = tie_kernel<double>(out);
         kern<<<(unsigned)blocks, 256, 0, st>>>(static_cast<const double *>(x), m->d, m->d_fit, m->d_y, m->n_train, k, m->n_classes,
                                                labels, scores, list, count, total, nb_ind, nb_dist);
     }
@@ -248,12 +234,12 @@ static int launch_marked(tcsdn_model *m, const void *x, int64_t n, int dtype, in
 
 int launch_knn_marked(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, double *scores,
                       const int32_t *list, const int *count, unsigned long long *total, cudaStream_t st) {
-    return launch_marked<false>(m, x, n, dtype, m->k, labels, scores, nullptr, nullptr, list, count, total, st);
+    return launch_marked(m, x, n, dtype, predict_out(m), m->k, labels, scores, nullptr, nullptr, list, count, total, st);
 }
 
 int launch_knn_marked_kneighbors(tcsdn_model *m, const void *x, int64_t n, int dtype, int nn, int64_t *ind, double *dist,
                                  const int32_t *list, const int *count, unsigned long long *total, cudaStream_t st) {
-    return launch_marked<true>(m, x, n, dtype, nn, nullptr, nullptr, ind, dist, list, count, total, st);
+    return launch_marked(m, x, n, dtype, KnnOut::Neighbors, nn, nullptr, nullptr, ind, dist, list, count, total, st);
 }
 
 }  // namespace tcsdn
