@@ -159,7 +159,7 @@ int tcsdn_predict(tcsdn_model_t *m, const void *x, int64_t n, int32_t d, int32_t
  * float32 rows are widened first.  1 <= n_neighbors <= min(64, n_samples_fit); TCSDN_EINVAL otherwise, for a handle that
  * is not a KNeighborsClassifier and under engine options 3 and 4.  Path, device, counters ([1] engine rows, [2] fp64
  * kernel rows, [7] index-order reruns) and non-finite rules are tcsdn_predict's: host pointers return TCSDN_ENONFINITE,
- * device pointers set the sticky flag tcsdn_sync_check reads.  Host pointers are processed one chunk at a time. */
+ * device pointers set the sticky flag tcsdn_sync_check reads.  Host pointers are processed through the same pipeline as tcsdn_predict. */
 int tcsdn_knn_kneighbors(tcsdn_model_t *m, const void *x, int64_t n, int32_t d, int32_t x_dtype, int32_t x_loc,
                          int32_t n_neighbors, int64_t *ind_out, double *dist_out /* nullable */, void *cuda_stream);
 

@@ -57,9 +57,11 @@ static bool finite_all(const double *p, size_t n) {
 
 static void free_workspace(Workspace *w) {
     for (int i = 0; i < 2; ++i) {
-        cudaFree(w->x[i].p); cudaFree(w->labels[i].p); cudaFree(w->scores[i].p);
-        if (w->h_labels[i]) cudaFreeHost(w->h_labels[i]);
-        if (w->h_scores[i]) cudaFreeHost(w->h_scores[i]);
+        cudaFree(w->x[i].p);
+        for (int j = 0; j < 2; ++j) {
+            cudaFree(w->out[i][j].p);
+            if (w->h_out[i][j]) cudaFreeHost(w->h_out[i][j]);
+        }
         if (w->stream[i]) cudaStreamDestroy(w->stream[i]);
         if (w->done[i]) cudaEventDestroy(w->done[i]);
     }
@@ -111,9 +113,21 @@ static void release_workspace(tcsdn_model *m, Workspace *w) {
     w->in_use = false;
 }
 
-// `flag`: where the kernels record non-finite rows -- the handle's sticky flag for device-pointer predicts (read by
-// tcsdn_sync_check), the workspace's own for host-pointer predicts (so that concurrent calls cannot see or clear
+// KNN predict and kneighbors: the engine when it can run the call, else the fp64 kernel (engine option 1 forces the latter).
+// `flag` (here and in run_device): where the kernels record non-finite rows -- the handle's sticky flag for device-pointer
+// calls (read by tcsdn_sync_check), the workspace's own for host-pointer calls (so that concurrent calls cannot see or clear
 // each other's)
+static int run_knn(tcsdn_model *m, const void *x, int64_t n, int dtype, const KnnCall &call, int32_t *flag, cudaStream_t st) {
+    if (!m->opt_check_finite) flag = nullptr;
+    if (m->opt_engine != 1 && knn_engine_usable(m, n, call)) return launch_knn_engine(m, x, n, dtype, call, flag, st);
+    if (m->opt_engine >= 2) {
+        set_error(call.out == KnnOut::Neighbors ? "tensor-core engine forced but not usable for this model/batch/n_neighbors"
+                                                : "tensor-core engine forced but not usable for this model/batch");
+        return TCSDN_EINVAL;
+    }
+    return launch_knn_exact(m, x, n, dtype, call, flag, st);
+}
+
 static int run_device(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, double *scores,
                       int32_t *flag, cudaStream_t st) {
     if (!m->opt_check_finite) flag = nullptr;
@@ -122,10 +136,7 @@ static int run_device(tcsdn_model *m, const void *x, int64_t n, int dtype, int32
         case TCSDN_KIND_GNB:
         case TCSDN_KIND_KMEANS: return launch_scorer(m, x, n, dtype, labels, scores, flag, st);
         case TCSDN_KIND_FOREST: return launch_forest(m, x, n, dtype, labels, scores, flag, st);
-        case TCSDN_KIND_KNN:
-            if (m->opt_engine != 1 && engine_usable(m, n, scores != nullptr)) return launch_knn_engine(m, x, n, dtype, labels, scores, flag, st);
-            if (m->opt_engine >= 2) { set_error("tensor-core engine forced but not usable for this model/batch"); return TCSDN_EINVAL; }
-            return launch_knn_exact(m, x, n, dtype, labels, scores, flag, st);
+        case TCSDN_KIND_KNN: return run_knn(m, x, n, dtype, KnnCall(m, labels, scores), flag, st);
         case TCSDN_KIND_SVC:
             // decision values are always the fp64 kernel's (the engine certifies LABELS; its fp32 sums cannot meet a
             // 1e-5 absolute bound on decision values, see dist_engine.cu)
@@ -137,13 +148,130 @@ static int run_device(tcsdn_model *m, const void *x, int64_t n, int dtype, int32
     return TCSDN_EINVAL;
 }
 
-// kneighbors: the same choice of path as a knn predict (the engine keeps at most 32 neighbours per query)
-static int run_kneighbors(tcsdn_model *m, const void *x, int64_t n, int dtype, int nn, int64_t *ind, double *dist,
-                          int32_t *flag, cudaStream_t st) {
-    if (!m->opt_check_finite) flag = nullptr;
-    if (m->opt_engine != 1 && engine_kneighbors_usable(m, n, nn)) return launch_knn_engine_kneighbors(m, x, n, dtype, nn, ind, dist, flag, st);
-    if (m->opt_engine == 2) { set_error("tensor-core engine forced but not usable for this model/batch/n_neighbors"); return TCSDN_EINVAL; }
-    return launch_knn_exact_kneighbors(m, x, n, dtype, nn, ind, dist, flag, st);
+int check_x(const tcsdn_model *m, int32_t d, int32_t x_dtype) {
+    if (d != m->d) {
+        set_error("X has %d features, but the model is expecting %d features as input", d, m->d);
+        return TCSDN_EINVAL;
+    }
+    if (x_dtype != TCSDN_F32 && x_dtype != TCSDN_F64) { set_error("x_dtype must be TCSDN_F32 or TCSDN_F64"); return TCSDN_EINVAL; }
+    return TCSDN_OK;
+}
+
+// the checks of a call on n rows of X whose one required output is `out` (named out_name in the message)
+static int check_call(const tcsdn_model *m, const void *x, int64_t n, int32_t d, int32_t x_dtype, int32_t x_loc, const void *out,
+                      const char *out_name) {
+    if (n < 0) { set_error("n must be >= 0"); return TCSDN_EINVAL; }
+    TCSDN_TRY(check_x(m, d, x_dtype));
+    if (x_loc != TCSDN_HOST && x_loc != TCSDN_DEVICE) { set_error("x_loc must be TCSDN_HOST or TCSDN_DEVICE"); return TCSDN_EINVAL; }
+    if (n > 0 && (!x || !out)) { set_error("x / %s is NULL", out_name); return TCSDN_EINVAL; }
+    return TCSDN_OK;
+}
+
+// gives the caller's current device back on every exit path of a call that begin_call moved to the handle's device
+struct DeviceGuard {
+    int prev = -1;
+    ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
+};
+
+// run on the handle's device and start the counters afresh: stats describe the last call
+static int begin_call(tcsdn_model *m, DeviceGuard &guard) {
+    int cur = -1;
+    TCSDN_CUDA(cudaGetDevice(&cur));
+    if (cur != m->dev) { TCSDN_CUDA(cudaSetDevice(m->dev)); guard.prev = cur; }
+    for (int i = 0; i < 8; ++i) m->stats[i].store(0, std::memory_order_relaxed);
+    return TCSDN_OK;
+}
+
+// rows per host-pipeline chunk for about `bytes` per chunk at `row_bytes` per row: a multiple of 1024, at least 1024
+static int64_t chunk_rows(size_t bytes, size_t row_bytes) {
+    return std::max<int64_t>(1024, (int64_t)(bytes / row_bytes) / 1024 * 1024);
+}
+
+// Host pointers: chunks of `chunk` rows (TCSDN_OPT_CHUNK_ROWS overrides it) alternate between two internal streams, so the
+// H2D copy of chunk c+1 runs under the kernels of chunk c and the D2H of chunk c-1 (PCIe is full duplex).
+// launch(x, rows, out0, out1, flag, st) enqueues one chunk's kernels on device buffers; the caller's out[i] receives
+// out_row[i] bytes per row (out[1] nullable).  Results go straight into the caller's arrays when those are page-locked
+// (cudaHostAlloc / cudaHostRegister).  With stage_pageable, pageable arrays are filled from pinned staging buffers (a D2H
+// copy into pageable memory blocks this thread until the chunk is done, which serialises the pipeline), memcpy'd to the
+// caller's arrays when their slot is recycled; without it, they too receive the D2H copy directly.
+template <typename Launch>
+static int run_host(tcsdn_model *m, const void *x, int64_t n, size_t row_bytes, int64_t chunk, void *const out[2],
+                    const size_t out_row[2], bool stage_pageable, const Launch &launch) {
+    if (m->opt_chunk_rows > 0) chunk = m->opt_chunk_rows;
+    if (chunk > n) chunk = n;
+    const int n_out = out[1] ? 2 : 1;
+    auto is_pinned = [](const void *p) {
+        cudaPointerAttributes a;
+        if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
+        return a.type == cudaMemoryTypeHost;
+    };
+    const bool direct_out = !stage_pageable || (is_pinned(out[0]) && (n_out == 1 || is_pinned(out[1])));
+    auto dst = [&](int i, int64_t row) { return static_cast<char *>(out[i]) + (size_t)row * out_row[i]; };
+    Workspace *w = nullptr;
+    TCSDN_TRY(acquire_workspace(m, &w));
+    int rc = TCSDN_OK;
+    int64_t pend_off[2] = {-1, -1}, pend_rows[2] = {0, 0};
+    auto drain = [&](int slot) -> int {   // wait for the slot's last chunk and hand its results to the caller
+        if (pend_off[slot] < 0) return TCSDN_OK;
+        cudaError_t e = cudaEventSynchronize(w->done[slot]);
+        if (e != cudaSuccess) { set_error("kernel execution failed: %s", cudaGetErrorString(e)); return TCSDN_ECUDA; }
+        if (!direct_out)
+            for (int i = 0; i < n_out; ++i) memcpy(dst(i, pend_off[slot]), w->h_out[slot][i], (size_t)pend_rows[slot] * out_row[i]);
+        pend_off[slot] = -1;
+        return TCSDN_OK;
+    };
+    do {
+        if (m->opt_check_finite) {
+            cudaError_t e = cudaMemsetAsync(w->d_flag, 0, sizeof(int32_t), w->stream[0]);
+            if (e == cudaSuccess) e = cudaEventRecord(w->done[1], w->stream[0]);
+            if (e == cudaSuccess) e = cudaStreamWaitEvent(w->stream[1], w->done[1], 0);
+            if (e != cudaSuccess) { set_error("flag reset failed: %s", cudaGetErrorString(e)); rc = TCSDN_ECUDA; break; }
+        }
+        int64_t done = 0;
+        int slot = 0;
+        while (done < n && rc == TCSDN_OK) {
+            const int64_t rows = (n - done) < chunk ? (n - done) : chunk;
+            cudaStream_t st = w->stream[slot];
+            if ((rc = drain(slot)) != TCSDN_OK) break;
+            if ((rc = ensure(w->x[slot], (size_t)chunk * row_bytes)) != TCSDN_OK) break;
+            for (int i = 0; i < n_out && rc == TCSDN_OK; ++i) {
+                rc = ensure(w->out[slot][i], (size_t)chunk * out_row[i]);
+                if (rc == TCSDN_OK && !direct_out) rc = ensure_pinned(&w->h_out[slot][i], &w->h_out_bytes[slot][i], (size_t)chunk * out_row[i]);
+            }
+            if (rc != TCSDN_OK) break;
+            cudaError_t e = cudaMemcpyAsync(w->x[slot].p, static_cast<const char *>(x) + (size_t)done * row_bytes,
+                                            (size_t)rows * row_bytes, cudaMemcpyHostToDevice, st);
+            if (e != cudaSuccess) { set_error("H2D copy failed: %s", cudaGetErrorString(e)); rc = TCSDN_ECUDA; break; }
+            rc = launch(w->x[slot].p, rows, w->out[slot][0].p, n_out == 2 ? w->out[slot][1].p : nullptr, w->d_flag, st);
+            if (rc != TCSDN_OK) break;
+            for (int i = 0; i < n_out && e == cudaSuccess; ++i)
+                e = cudaMemcpyAsync(direct_out ? dst(i, done) : w->h_out[slot][i], w->out[slot][i].p, (size_t)rows * out_row[i],
+                                    cudaMemcpyDeviceToHost, st);
+            if (e == cudaSuccess) e = cudaEventRecord(w->done[slot], st);
+            if (e != cudaSuccess) { set_error("D2H copy failed: %s", cudaGetErrorString(e)); rc = TCSDN_ECUDA; break; }
+            pend_off[slot] = done; pend_rows[slot] = rows;
+            done += rows;
+            slot ^= 1;
+        }
+        for (int i = 0; i < 2; ++i) {   // oldest first
+            int r2 = drain(slot ^ i);
+            if (rc == TCSDN_OK) rc = r2;
+        }
+        for (int i = 0; i < 2; ++i) {
+            cudaError_t e = cudaStreamSynchronize(w->stream[i]);
+            if (e != cudaSuccess && rc == TCSDN_OK) { set_error("kernel execution failed: %s", cudaGetErrorString(e)); rc = TCSDN_ECUDA; }
+        }
+        if (rc == TCSDN_OK && m->opt_check_finite) {
+            cudaError_t e = cudaMemcpy(w->h_flag, w->d_flag, sizeof(int32_t), cudaMemcpyDeviceToHost);
+            if (e != cudaSuccess) { set_error("flag read failed: %s", cudaGetErrorString(e)); rc = TCSDN_ECUDA; }
+            else if (*w->h_flag) {
+                set_error("Input X contains NaN or infinity");
+                rc = TCSDN_ENONFINITE;
+            }
+        }
+    } while (0);
+    release_workspace(m, w);
+    return rc;
 }
 
 }  // namespace tcsdn
@@ -423,129 +551,25 @@ int tcsdn_model_stats(const tcsdn_model_t *m, int64_t *out) {
 int tcsdn_predict(tcsdn_model_t *m, const void *x, int64_t n, int32_t d, int32_t x_dtype, int32_t x_loc,
                   int32_t *labels_out, double *scores_out, void *cuda_stream) {
     if (!m) { set_error("model is NULL"); return TCSDN_EINVAL; }
-    if (n < 0) { set_error("n must be >= 0"); return TCSDN_EINVAL; }
-    if (d != m->d) {
-        set_error("X has %d features, but the model is expecting %d features as input", d, m->d);
-        return TCSDN_EINVAL;
-    }
-    if (x_dtype != TCSDN_F32 && x_dtype != TCSDN_F64) { set_error("x_dtype must be TCSDN_F32 or TCSDN_F64"); return TCSDN_EINVAL; }
-    if (x_loc != TCSDN_HOST && x_loc != TCSDN_DEVICE) { set_error("x_loc must be TCSDN_HOST or TCSDN_DEVICE"); return TCSDN_EINVAL; }
+    TCSDN_TRY(check_call(m, x, n, d, x_dtype, x_loc, labels_out, "labels_out"));
     if (n == 0) return TCSDN_OK;
-    if (!x || !labels_out) { set_error("x / labels_out is NULL"); return TCSDN_EINVAL; }
-    // run on the handle's device and give the caller's current device back on every exit path
-    struct DeviceGuard {
-        int prev = -1;
-        ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
-    } guard;
-    int cur = -1;
-    TCSDN_CUDA(cudaGetDevice(&cur));
-    if (cur != m->dev) { TCSDN_CUDA(cudaSetDevice(m->dev)); guard.prev = cur; }
-    for (int i = 0; i < 8; ++i) m->stats[i].store(0, std::memory_order_relaxed);
-
+    DeviceGuard guard;
+    TCSDN_TRY(begin_call(m, guard));
     if (x_loc == TCSDN_DEVICE) {
         // the non-finite flag is sticky on this path: kernels only OR into it, tcsdn_sync_check reads and clears it
         // (no memset node per predict: a 1M-row predict lasts microseconds)
         return run_device(m, x, n, x_dtype, labels_out, scores_out, m->d_flag, static_cast<cudaStream_t>(cuda_stream));
     }
-
-    // host pointers: chunks alternate between two internal streams, so the H2D copy of chunk c+1 runs under the
-    // kernels of chunk c and the D2H of chunk c-1 (PCIe is full duplex).  Results land in pinned staging
-    // buffers (a D2H copy into pageable memory would block this thread and serialise the pipeline) and are
-    // memcpy'd to the caller's arrays when their slot is recycled.
-    const size_t esz = x_dtype == TCSDN_F32 ? 4 : 8;
-    const size_t row_bytes = (size_t)d * esz;
-    int64_t chunk = m->opt_chunk_rows;
-    if (chunk <= 0) {
-        // ~16 MiB of rows per chunk for the streaming kernels (the copy is their bottleneck: small chunks start the overlap early);
-        // 128 MiB for the distance engine, whose persistent CTAs take 256 rows per pass and want several passes per launch
-        const size_t chunk_bytes = (m->kind == TCSDN_KIND_KNN || m->kind == TCSDN_KIND_SVC) ? (128u << 20) : (16u << 20);
-        chunk = (int64_t)(chunk_bytes / row_bytes);
-        chunk = (chunk / 1024) * 1024;
-        if (chunk < 1024) chunk = 1024;
-    }
-    if (chunk > n) chunk = n;
-    const size_t sc_cols = scores_out ? (size_t)m->score_cols : 0;
-    // results go straight into the caller's arrays when those are page-locked (cudaHostAlloc / cudaHostRegister);
-    // pageable arrays are filled from pinned staging buffers
-    auto is_pinned = [](const void *p) {
-        cudaPointerAttributes a;
-        if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
-        return a.type == cudaMemoryTypeHost;
-    };
-    const bool direct_out = is_pinned(labels_out) && (!sc_cols || is_pinned(scores_out));
-    Workspace *w = nullptr;
-    TCSDN_TRY(acquire_workspace(m, &w));
-    int rc = TCSDN_OK;
-    int64_t pend_off[2] = {-1, -1}, pend_rows[2] = {0, 0};
-    auto drain = [&](int slot) -> int {   // wait for the slot's last chunk and hand its results to the caller
-        if (pend_off[slot] < 0) return TCSDN_OK;
-        cudaError_t e = cudaEventSynchronize(w->done[slot]);
-        if (e != cudaSuccess) { set_error("kernel execution failed: %s", cudaGetErrorString(e)); return TCSDN_ECUDA; }
-        if (!direct_out) {
-            memcpy(labels_out + pend_off[slot], w->h_labels[slot], (size_t)pend_rows[slot] * sizeof(int32_t));
-            if (sc_cols)
-                memcpy(scores_out + (size_t)pend_off[slot] * sc_cols, w->h_scores[slot],
-                       (size_t)pend_rows[slot] * sc_cols * sizeof(double));
-        }
-        pend_off[slot] = -1;
-        return TCSDN_OK;
-    };
-    do {
-        if (m->opt_check_finite) {
-            cudaError_t e = cudaMemsetAsync(w->d_flag, 0, sizeof(int32_t), w->stream[0]);
-            if (e == cudaSuccess) e = cudaEventRecord(w->done[1], w->stream[0]);
-            if (e == cudaSuccess) e = cudaStreamWaitEvent(w->stream[1], w->done[1], 0);
-            if (e != cudaSuccess) { set_error("flag reset failed: %s", cudaGetErrorString(e)); rc = TCSDN_ECUDA; break; }
-        }
-        int64_t done = 0;
-        int slot = 0;
-        while (done < n && rc == TCSDN_OK) {
-            const int64_t rows = (n - done) < chunk ? (n - done) : chunk;
-            cudaStream_t st = w->stream[slot];
-            if ((rc = drain(slot)) != TCSDN_OK) break;
-            if ((rc = ensure(w->x[slot], (size_t)chunk * row_bytes)) != TCSDN_OK) break;
-            if ((rc = ensure(w->labels[slot], (size_t)chunk * sizeof(int32_t))) != TCSDN_OK) break;
-            if (!direct_out && (rc = ensure_pinned(&w->h_labels[slot], &w->h_labels_bytes[slot], (size_t)chunk * sizeof(int32_t))) != TCSDN_OK) break;
-            if (sc_cols) {
-                if ((rc = ensure(w->scores[slot], (size_t)chunk * sc_cols * sizeof(double))) != TCSDN_OK) break;
-                if (!direct_out && (rc = ensure_pinned(&w->h_scores[slot], &w->h_scores_bytes[slot], (size_t)chunk * sc_cols * sizeof(double))) != TCSDN_OK) break;
-            }
-            cudaError_t e = cudaMemcpyAsync(w->x[slot].p, static_cast<const char *>(x) + (size_t)done * row_bytes,
-                                            (size_t)rows * row_bytes, cudaMemcpyHostToDevice, st);
-            if (e != cudaSuccess) { set_error("H2D copy failed: %s", cudaGetErrorString(e)); rc = TCSDN_ECUDA; break; }
-            rc = run_device(m, w->x[slot].p, rows, x_dtype, static_cast<int32_t *>(w->labels[slot].p),
-                            sc_cols ? static_cast<double *>(w->scores[slot].p) : nullptr, w->d_flag, st);
-            if (rc != TCSDN_OK) break;
-            e = cudaMemcpyAsync(direct_out ? (void *)(labels_out + done) : w->h_labels[slot], w->labels[slot].p,
-                                (size_t)rows * sizeof(int32_t), cudaMemcpyDeviceToHost, st);
-            if (e == cudaSuccess && sc_cols)
-                e = cudaMemcpyAsync(direct_out ? (void *)(scores_out + (size_t)done * sc_cols) : w->h_scores[slot],
-                                    w->scores[slot].p, (size_t)rows * sc_cols * sizeof(double), cudaMemcpyDeviceToHost, st);
-            if (e == cudaSuccess) e = cudaEventRecord(w->done[slot], st);
-            if (e != cudaSuccess) { set_error("D2H copy failed: %s", cudaGetErrorString(e)); rc = TCSDN_ECUDA; break; }
-            pend_off[slot] = done; pend_rows[slot] = rows;
-            done += rows;
-            slot ^= 1;
-        }
-        for (int i = 0; i < 2; ++i) {   // oldest first
-            int r2 = drain(slot ^ i ^ 0);
-            if (rc == TCSDN_OK) rc = r2;
-        }
-        for (int i = 0; i < 2; ++i) {
-            cudaError_t e = cudaStreamSynchronize(w->stream[i]);
-            if (e != cudaSuccess && rc == TCSDN_OK) { set_error("kernel execution failed: %s", cudaGetErrorString(e)); rc = TCSDN_ECUDA; }
-        }
-        if (rc == TCSDN_OK && m->opt_check_finite) {
-            cudaError_t e = cudaMemcpy(w->h_flag, w->d_flag, sizeof(int32_t), cudaMemcpyDeviceToHost);
-            if (e != cudaSuccess) { set_error("flag read failed: %s", cudaGetErrorString(e)); rc = TCSDN_ECUDA; }
-            else if (*w->h_flag) {
-                set_error("Input X contains NaN or infinity");
-                rc = TCSDN_ENONFINITE;
-            }
-        }
-    } while (0);
-    release_workspace(m, w);
-    return rc;
+    // ~16 MiB of rows per chunk for the streaming kernels (the copy is their bottleneck: small chunks start the overlap early);
+    // 128 MiB for the distance engine, whose persistent CTAs take 256 rows per pass and want several passes per launch
+    const size_t row_bytes = (size_t)d * (x_dtype == TCSDN_F32 ? 4 : 8);
+    const size_t chunk_bytes = (m->kind == TCSDN_KIND_KNN || m->kind == TCSDN_KIND_SVC) ? (128u << 20) : (16u << 20);
+    void *const out[2] = {labels_out, scores_out};
+    const size_t out_row[2] = {sizeof(int32_t), scores_out ? (size_t)m->score_cols * sizeof(double) : 0};
+    return run_host(m, x, n, row_bytes, chunk_rows(chunk_bytes, row_bytes), out, out_row, true,
+                    [&](const void *xc, int64_t rows, void *labels, void *scores, int32_t *flag, cudaStream_t st) {
+                        return run_device(m, xc, rows, x_dtype, static_cast<int32_t *>(labels), static_cast<double *>(scores), flag, st);
+                    });
 }
 
 int tcsdn_knn_kneighbors(tcsdn_model_t *m, const void *x, int64_t n, int32_t d, int32_t x_dtype, int32_t x_loc,
@@ -558,69 +582,23 @@ int tcsdn_knn_kneighbors(tcsdn_model_t *m, const void *x, int64_t n, int32_t d, 
         return TCSDN_EINVAL;
     }
     if (m->opt_engine >= 3) { set_error("kneighbors: engine options 3 and 4 are predict audits"); return TCSDN_EINVAL; }
-    if (n < 0) { set_error("n must be >= 0"); return TCSDN_EINVAL; }
-    if (d != m->d) {
-        set_error("X has %d features, but the model is expecting %d features as input", d, m->d);
-        return TCSDN_EINVAL;
-    }
-    if (x_dtype != TCSDN_F32 && x_dtype != TCSDN_F64) { set_error("x_dtype must be TCSDN_F32 or TCSDN_F64"); return TCSDN_EINVAL; }
-    if (x_loc != TCSDN_HOST && x_loc != TCSDN_DEVICE) { set_error("x_loc must be TCSDN_HOST or TCSDN_DEVICE"); return TCSDN_EINVAL; }
+    TCSDN_TRY(check_call(m, x, n, d, x_dtype, x_loc, ind_out, "ind_out"));
     if (n == 0) return TCSDN_OK;
-    if (!x || !ind_out) { set_error("x / ind_out is NULL"); return TCSDN_EINVAL; }
-    struct DeviceGuard {
-        int prev = -1;
-        ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
-    } guard;
-    int cur = -1;
-    TCSDN_CUDA(cudaGetDevice(&cur));
-    if (cur != m->dev) { TCSDN_CUDA(cudaSetDevice(m->dev)); guard.prev = cur; }
-    for (int i = 0; i < 8; ++i) m->stats[i].store(0, std::memory_order_relaxed);
-    const int nn = n_neighbors;
+    DeviceGuard guard;
+    TCSDN_TRY(begin_call(m, guard));
     if (x_loc == TCSDN_DEVICE)   // sticky non-finite flag, read by tcsdn_sync_check (as for tcsdn_predict)
-        return run_kneighbors(m, x, n, x_dtype, nn, ind_out, dist_out, m->d_flag, static_cast<cudaStream_t>(cuda_stream));
-
-    // host pointers: one chunk at a time on one internal stream (copy in, kernels, copy out, wait)
+        return run_knn(m, x, n, x_dtype, KnnCall(n_neighbors, ind_out, dist_out), m->d_flag, static_cast<cudaStream_t>(cuda_stream));
+    // ~128 MiB of rows and results per chunk.  The results take up to 1 KiB per row, so pageable arrays are not staged: the
+    // second host copy costs more than its overlap saves (1M float32 rows, n_neighbors = 5: one chunk, 58 ms a call written
+    // directly, 69-88 ms staged; H100 80GB HBM3 at 700 W)
     const size_t row_bytes = (size_t)d * (x_dtype == TCSDN_F32 ? 4 : 8);
-    const size_t out_row = (size_t)nn * sizeof(int64_t), dist_row = dist_out ? (size_t)nn * sizeof(double) : 0;
-    int64_t chunk = m->opt_chunk_rows;
-    if (chunk <= 0) {
-        chunk = (int64_t)((128u << 20) / (row_bytes + out_row + dist_row));
-        chunk = std::max<int64_t>(1024, (chunk / 1024) * 1024);
-    }
-    if (chunk > n) chunk = n;
-    Workspace *w = nullptr;
-    TCSDN_TRY(acquire_workspace(m, &w));
-    cudaStream_t st = w->stream[0];
-    int rc = ensure(w->x[0], (size_t)chunk * row_bytes);
-    if (rc == TCSDN_OK) rc = ensure(w->labels[0], (size_t)chunk * out_row);   // the workspace's label buffer holds ind here
-    if (rc == TCSDN_OK && dist_out) rc = ensure(w->scores[0], (size_t)chunk * dist_row);
-    if (rc == TCSDN_OK && m->opt_check_finite && cudaMemsetAsync(w->d_flag, 0, sizeof(int32_t), st) != cudaSuccess) {
-        set_error("flag reset failed");
-        rc = TCSDN_ECUDA;
-    }
-    for (int64_t done = 0; done < n && rc == TCSDN_OK;) {
-        const int64_t rows = std::min<int64_t>(chunk, n - done);
-        cudaError_t e = cudaMemcpyAsync(w->x[0].p, static_cast<const char *>(x) + (size_t)done * row_bytes, (size_t)rows * row_bytes,
-                                        cudaMemcpyHostToDevice, st);
-        if (e != cudaSuccess) { set_error("H2D copy failed: %s", cudaGetErrorString(e)); rc = TCSDN_ECUDA; break; }
-        rc = run_kneighbors(m, w->x[0].p, rows, x_dtype, nn, static_cast<int64_t *>(w->labels[0].p),
-                            dist_out ? static_cast<double *>(w->scores[0].p) : nullptr, w->d_flag, st);
-        if (rc != TCSDN_OK) break;
-        e = cudaMemcpyAsync(ind_out + (size_t)done * nn, w->labels[0].p, (size_t)rows * out_row, cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess && dist_out)
-            e = cudaMemcpyAsync(dist_out + (size_t)done * nn, w->scores[0].p, (size_t)rows * dist_row, cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-        if (e != cudaSuccess) { set_error("kneighbors failed: %s", cudaGetErrorString(e)); rc = TCSDN_ECUDA; break; }
-        done += rows;
-    }
-    if (rc != TCSDN_OK) cudaStreamSynchronize(st);   // nothing of this call may still run when the workspace is reused
-    if (rc == TCSDN_OK && m->opt_check_finite) {
-        cudaError_t e = cudaMemcpy(w->h_flag, w->d_flag, sizeof(int32_t), cudaMemcpyDeviceToHost);
-        if (e != cudaSuccess) { set_error("flag read failed: %s", cudaGetErrorString(e)); rc = TCSDN_ECUDA; }
-        else if (*w->h_flag) { set_error("Input X contains NaN or infinity"); rc = TCSDN_ENONFINITE; }
-    }
-    release_workspace(m, w);
-    return rc;
+    void *const out[2] = {ind_out, dist_out};
+    const size_t out_row[2] = {(size_t)n_neighbors * sizeof(int64_t), dist_out ? (size_t)n_neighbors * sizeof(double) : 0};
+    return run_host(m, x, n, row_bytes, chunk_rows(128u << 20, row_bytes + out_row[0] + out_row[1]), out, out_row, false,
+                    [&](const void *xc, int64_t rows, void *ind, void *dist, int32_t *flag, cudaStream_t st) {
+                        return run_knn(m, xc, rows, x_dtype, KnnCall(n_neighbors, static_cast<int64_t *>(ind), static_cast<double *>(dist)),
+                                       flag, st);
+                    });
 }
 
 int tcsdn_sync_check(tcsdn_model_t *m, void *cuda_stream) {

@@ -316,8 +316,7 @@ int tcsdn_comm_gather_buffer(tcsdn_comm_t *c, int64_t n_block, const uint8_t **g
 int tcsdn_predict_gathered(tcsdn_model_t *m, tcsdn_comm_t *c, const void *x, int64_t n_local, int32_t d, int32_t x_dtype,
                            const uint8_t **gathered_out, void *cuda_stream) {
     if (!m || !c || n_local < 0 || (n_local > 0 && !x)) { set_error("predict_gathered: bad arguments"); return TCSDN_EINVAL; }
-    if (d != m->d) { set_error("X has %d features, but the model is expecting %d features as input", d, m->d); return TCSDN_EINVAL; }
-    if (x_dtype != TCSDN_F32 && x_dtype != TCSDN_F64) { set_error("x_dtype must be TCSDN_F32 or TCSDN_F64"); return TCSDN_EINVAL; }
+    TCSDN_TRY(check_x(m, d, x_dtype));
     if (m->n_classes > 255 && m->kind != TCSDN_KIND_FOREST && m->kind != TCSDN_KIND_KNN && m->kind != TCSDN_KIND_SVC) {
         set_error("predict_gathered: labels travel as bytes, the model has %d classes", m->n_classes); return TCSDN_EINVAL; }
     if (!c->g_peer[c->rank] || n_local > c->g_block) { set_error("predict_gathered: call tcsdn_comm_gather_buffer(n_block >= %lld) first", (long long)n_local); return TCSDN_EINVAL; }

@@ -241,11 +241,10 @@ struct DeviceBuf {
     size_t bytes = 0;
 };
 
-struct Workspace {  // per-call scratch for the host-pointer pipeline
-    DeviceBuf x[2], labels[2], scores[2];
-    void *h_labels[2] = {nullptr, nullptr};   // pinned D2H staging (results are memcpy'd to the caller's buffer)
-    void *h_scores[2] = {nullptr, nullptr};
-    size_t h_labels_bytes[2] = {0, 0}, h_scores_bytes[2] = {0, 0};
+struct Workspace {  // per-call scratch for the host-pointer pipeline, two slots
+    DeviceBuf x[2], out[2][2];                 // [slot]: the rows; [slot][i]: the call's output i (labels / ind, scores / dist)
+    void *h_out[2][2] = {};                    // pinned D2H staging (results are memcpy'd to the caller's buffer)
+    size_t h_out_bytes[2][2] = {};
     cudaStream_t stream[2] = {nullptr, nullptr};
     cudaEvent_t done[2] = {nullptr, nullptr};
     int32_t *h_flag = nullptr;  // pinned
@@ -315,23 +314,34 @@ struct tcsdn_model {
 
 namespace tcsdn {
 
+// One KNN call as the host launchers see it (it never reaches the device).  predict: the handle's vote over its k neighbours
+// into labels [n] and scores [n][C] (nullable); kneighbors: the k = n_neighbors nearest training rows, ind [n][k] and dist
+// [n][k] (nullable), in ascending (distance, index) order -- the set is sklearn's index-order heap's, as for predict.
+struct KnnCall {
+    KnnOut out;
+    int k;
+    int32_t *labels = nullptr;
+    double *scores = nullptr;
+    int64_t *ind = nullptr;
+    double *dist = nullptr;
+    KnnCall(const tcsdn_model *m, int32_t *labels_, double *scores_)   // the distance-weighted vote is weights='distance''s
+        : out(m->knn_weights == TCSDN_KNN_DISTANCE ? KnnOut::WeightedVote : KnnOut::Vote), k(m->k), labels(labels_), scores(scores_) {}
+    KnnCall(int n_neighbors, int64_t *ind_, double *dist_) : out(KnnOut::Neighbors), k(n_neighbors), ind(ind_), dist(dist_) {}
+};
+
+// tcsdn_predict's argument checks shared by every entry that takes rows of X: the feature count and the dtype
+int check_x(const tcsdn_model *m, int32_t d, int32_t x_dtype);
+
 // kernels' host launchers (each enqueues on `st`, returns TCSDN_*).  x is a DEVICE pointer.
 // `flag` (nullable): device int32 the kernels OR 1 into when a row holds NaN/inf.
 int launch_scorer(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, double *scores,
                   int32_t *flag, cudaStream_t st, const GatherOut *gather = nullptr);
 int launch_forest(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, double *scores,
                   int32_t *flag, cudaStream_t st);
-int launch_knn_exact(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, double *scores,
-                     int32_t *flag, cudaStream_t st);
+int launch_knn_exact(tcsdn_model *m, const void *x, int64_t n, int dtype, const KnnCall &call, int32_t *flag, cudaStream_t st);
 // the rows listed in list[0 .. *count) only (the knn engine's tie rows); *count is added to *total
-int launch_knn_marked(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, double *scores,
-                      const int32_t *list, const int *count, unsigned long long *total, cudaStream_t st);
-// KNeighbors.kneighbors: per row the nn nearest training rows, ind [n][nn] int64 and dist [n][nn] (nullable), in
-// ascending (distance, index) order; the set is sklearn's index-order heap's, as for predict
-int launch_knn_exact_kneighbors(tcsdn_model *m, const void *x, int64_t n, int dtype, int nn, int64_t *ind, double *dist,
-                                int32_t *flag, cudaStream_t st);
-int launch_knn_marked_kneighbors(tcsdn_model *m, const void *x, int64_t n, int dtype, int nn, int64_t *ind, double *dist,
-                                 const int32_t *list, const int *count, unsigned long long *total, cudaStream_t st);
+int launch_knn_marked(tcsdn_model *m, const void *x, int64_t n, int dtype, const KnnCall &call, const int32_t *list,
+                      const int *count, unsigned long long *total, cudaStream_t st);
 int launch_svc_exact(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, double *scores,
                      int32_t *flag, cudaStream_t st);
 int launch_ovr_from_ovo(const double *dec, int64_t n, int C, double *out, cudaStream_t st);
@@ -347,18 +357,15 @@ int knn_engine_create(tcsdn_model *m);
 int svc_engine_create(tcsdn_model *m);
 void engine_destroy(tcsdn_model *m);
 bool engine_usable(const tcsdn_model *m, int64_t n, bool want_scores);
+bool knn_engine_usable(const tcsdn_model *m, int64_t n, const KnnCall &call);
 void engine_read_stats(const tcsdn_model *m, int64_t *out8);
 // svc.cu: re-evaluate, in fp64, exactly the rows whose label is negative (-1 - label, left by the engine's certificate);
 // `counter` (device) receives the number of such rows
 int launch_svc_marked(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, unsigned long long *counter,
                       cudaStream_t st);
-int launch_knn_engine(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, double *scores,
-                      int32_t *flag, cudaStream_t st);
+int launch_knn_engine(tcsdn_model *m, const void *x, int64_t n, int dtype, const KnnCall &call, int32_t *flag, cudaStream_t st);
 int launch_svc_engine(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, double *scores,
                       int32_t *flag, cudaStream_t st);
-bool engine_kneighbors_usable(const tcsdn_model *m, int64_t n, int nn);
-int launch_knn_engine_kneighbors(tcsdn_model *m, const void *x, int64_t n, int dtype, int nn, int64_t *ind, double *dist,
-                                 int32_t *flag, cudaStream_t st);
 
 template <typename T>
 int upload(T **dst, const T *src, size_t count) {

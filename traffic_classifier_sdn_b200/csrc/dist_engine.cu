@@ -1692,19 +1692,16 @@ static auto knn_kernel(bool heap_smem) {
     return heap_smem ? knn_engine_kernel<T, true, AUDIT, OUT> : knn_engine_kernel<T, false, AUDIT, OUT>;
 }
 
-// kk: neighbours kept per query (the model's k for predict, the call's n_neighbors for kneighbors); KnnOut::Neighbors writes
-// nb_ind / nb_dist instead of labels / scores
 template <typename T>
-static int knn_engine_run(tcsdn_model *m, const T *x, int64_t n, int32_t *labels, double *scores, int32_t *flag,
-                          cudaStream_t st, KnnOut out, int kk, int64_t *nb_ind, double *nb_dist) {
+static int knn_engine_run(tcsdn_model *m, const T *x, int64_t n, const KnnCall &call, int32_t *flag, cudaStream_t st) {
     KnnEngine *E = static_cast<KnnEngine *>(m->engine);
     KnnArgs A;
     common_args(A, m, E, n, flag);
-    A.tile_rows = E->d_tile_rows; A.y = m->d_y; A.k = kk; A.C = m->n_classes;
-    A.pos_orig = E->d_pos_orig; A.nb_ind = nb_ind; A.nb_dist = nb_dist;
+    A.tile_rows = E->d_tile_rows; A.y = m->d_y; A.k = call.k; A.C = m->n_classes;
+    A.pos_orig = E->d_pos_orig; A.nb_ind = call.ind; A.nb_dist = call.dist;
     A.refpad = E->d_refpad; A.dpad = kEMaxD;
     A.flush_tiles = m->opt_knn_flush > 0 ? (int)m->opt_knn_flush : kEFlushTiles;   // TCSDN_OPT_KNN_FLUSH_TILES
-    const bool heap_smem = kk <= kEHeapSmemK;
+    const bool heap_smem = call.k <= kEHeapSmemK;
     // Order the queries by home tile (counting sort on this stream) so that a pass's 256 rows are neighbours and the
     // producer can leave out the tiles that are too far for all of them.  Scratch comes from the engine's own stream-ordered
     // pool (capturable into a CUDA graph, private to the call).
@@ -1745,28 +1742,25 @@ static int knn_engine_run(tcsdn_model *m, const T *x, int64_t n, int32_t *labels
         A.qperm = perm; A.qkey = key; A.leaf_tile = E->d_leaf_tile;
     }
     const size_t smem = e_smem_bytes(E->tile_bytes) + kERows * (size_t)kEListCap * sizeof(uint16_t) +
-                        (heap_smem ? kERows * (size_t)kk * 12 : 0);
+                        (heap_smem ? kERows * (size_t)call.k * 12 : 0);
     decltype(&knn_engine_kernel<T, false, false, KnnOut::Vote>) kern;
     if (A.maxratio) {
-        if (out != KnnOut::Vote) { set_error("knn engine: kneighbors and distance weights have no audit mode"); return TCSDN_EINVAL; }
+        if (call.out != KnnOut::Vote) { set_error("knn engine: kneighbors and distance weights have no audit mode"); return TCSDN_EINVAL; }
         kern = knn_kernel<T, true, KnnOut::Vote>(heap_smem);
-    } else if (out == KnnOut::Vote) {
+    } else if (call.out == KnnOut::Vote) {
         kern = knn_kernel<T, false, KnnOut::Vote>(heap_smem);
-    } else if (out == KnnOut::WeightedVote) {
+    } else if (call.out == KnnOut::WeightedVote) {
         kern = knn_kernel<T, false, KnnOut::WeightedVote>(heap_smem);
     } else {
         kern = knn_kernel<T, false, KnnOut::Neighbors>(heap_smem);
     }
     TCSDN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kern<<<engine_grid(m, n), kEKnnThreads, smem, st>>>(A, x, labels, scores, E->d_counters);
+    kern<<<engine_grid(m, n), kEKnnThreads, smem, st>>>(A, x, call.labels, call.scores, E->d_counters);
     TCSDN_CUDA(cudaGetLastError());
     m->stats[0] += 1;
     m->stats[1] += n;
     // rows whose result hangs on a tie at the k-th distance get sklearn's index-order heap (knn.cu), on the same stream
-    const int dtype = sizeof(T) == 4 ? TCSDN_F32 : TCSDN_F64;
-    if (out == KnnOut::Neighbors)
-        return launch_knn_marked_kneighbors(m, x, n, dtype, kk, nb_ind, nb_dist, A.tie_list, A.tie_count, E->d_counters + 1, st);
-    return launch_knn_marked(m, x, n, dtype, labels, scores, A.tie_list, A.tie_count, E->d_counters + 1, st);
+    return launch_knn_marked(m, x, n, sizeof(T) == 4 ? TCSDN_F32 : TCSDN_F64, call, A.tie_list, A.tie_count, E->d_counters + 1, st);
 }
 
 template <typename T, int NC1>
@@ -1808,25 +1802,15 @@ static int svc_engine_run(tcsdn_model *m, const T *x, int64_t n, int32_t *labels
     return TCSDN_OK;
 }
 
-int launch_knn_engine(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, double *scores, int32_t *flag,
-                      cudaStream_t st) {
-    if (n == 0) return TCSDN_OK;
-    // the distance-weighted vote belongs to predict on weights='distance' handles
-    const KnnOut out = m->knn_weights == TCSDN_KNN_DISTANCE ? KnnOut::WeightedVote : KnnOut::Vote;
-    if (dtype == TCSDN_F32) return knn_engine_run<float>(m, static_cast<const float *>(x), n, labels, scores, flag, st, out, m->k, nullptr, nullptr);
-    return knn_engine_run<double>(m, static_cast<const double *>(x), n, labels, scores, flag, st, out, m->k, nullptr, nullptr);
+// the engine keeps at most kEMaxK neighbours per query (a handle with a larger k has no engine)
+bool knn_engine_usable(const tcsdn_model *m, int64_t n, const KnnCall &call) {
+    return call.k <= kEMaxK && engine_usable(m, n, call.scores != nullptr);
 }
 
-bool engine_kneighbors_usable(const tcsdn_model *m, int64_t n, int nn) {
-    return m->kind == TCSDN_KIND_KNN && nn <= kEMaxK && engine_usable(m, n, false);
-}
-
-int launch_knn_engine_kneighbors(tcsdn_model *m, const void *x, int64_t n, int dtype, int nn, int64_t *ind, double *dist,
-                                 int32_t *flag, cudaStream_t st) {
+int launch_knn_engine(tcsdn_model *m, const void *x, int64_t n, int dtype, const KnnCall &call, int32_t *flag, cudaStream_t st) {
     if (n == 0) return TCSDN_OK;
-    if (dtype == TCSDN_F32)
-        return knn_engine_run<float>(m, static_cast<const float *>(x), n, nullptr, nullptr, flag, st, KnnOut::Neighbors, nn, ind, dist);
-    return knn_engine_run<double>(m, static_cast<const double *>(x), n, nullptr, nullptr, flag, st, KnnOut::Neighbors, nn, ind, dist);
+    if (dtype == TCSDN_F32) return knn_engine_run<float>(m, static_cast<const float *>(x), n, call, flag, st);
+    return knn_engine_run<double>(m, static_cast<const double *>(x), n, call, flag, st);
 }
 
 int launch_svc_engine(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, double *scores, int32_t *flag,

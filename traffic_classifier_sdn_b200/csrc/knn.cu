@@ -23,11 +23,6 @@ constexpr int kKnnThreads = 128;
 constexpr int kKnnTile = 128;    // training rows per shared-memory tile
 constexpr int kKnnMaxK = 64;
 
-// the distance-weighted vote is a predict mode of weights='distance' handles; kneighbors has no vote
-static KnnOut predict_out(const tcsdn_model *m) {
-    return m->knn_weights == TCSDN_KNN_DISTANCE ? KnnOut::WeightedVote : KnnOut::Vote;
-}
-
 __device__ __forceinline__ void heap_push_dev(double *values, int32_t *indices, int size, double val, int32_t val_idx) {
     // caller has already checked val < values[0]
     values[0] = val;
@@ -107,9 +102,7 @@ static auto exact_kernel(KnnOut out) {
                                          : knn_exact_kernel<T, KnnOut::Vote>;
 }
 
-// predict (labels / scores, the model's k) or kneighbors (nb_ind / nb_dist, k = the call's n_neighbors)
-static int launch_exact(tcsdn_model *m, const void *x, int64_t n, int dtype, KnnOut out, int k, int32_t *labels, double *scores,
-                        int64_t *nb_ind, double *nb_dist, int32_t *flag, cudaStream_t st) {
+int launch_knn_exact(tcsdn_model *m, const void *x, int64_t n, int dtype, const KnnCall &call, int32_t *flag, cudaStream_t st) {
     if (n == 0) return TCSDN_OK;
     const size_t smem = ((size_t)m->d * kKnnThreads + (size_t)kKnnTile * m->d) * sizeof(double);
     int64_t blocks = (n + kKnnThreads - 1) / kKnnThreads;
@@ -118,28 +111,18 @@ static int launch_exact(tcsdn_model *m, const void *x, int64_t n, int dtype, Knn
     m->stats[0] += 1;
     m->stats[2] += n;
     if (dtype == TCSDN_F32) {
-        auto kern = exact_kernel<float>(out);
+        auto kern = exact_kernel<float>(call.out);
         TCSDN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        kern<<<(unsigned)blocks, kKnnThreads, smem, st>>>(static_cast<const float *>(x), n, m->d, m->d_fit, m->d_y,
-                                                          m->n_train, k, m->n_classes, labels, scores, flag, nb_ind, nb_dist);
+        kern<<<(unsigned)blocks, kKnnThreads, smem, st>>>(static_cast<const float *>(x), n, m->d, m->d_fit, m->d_y, m->n_train,
+                                                          call.k, m->n_classes, call.labels, call.scores, flag, call.ind, call.dist);
     } else {
-        auto kern = exact_kernel<double>(out);
+        auto kern = exact_kernel<double>(call.out);
         TCSDN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        kern<<<(unsigned)blocks, kKnnThreads, smem, st>>>(static_cast<const double *>(x), n, m->d, m->d_fit, m->d_y,
-                                                          m->n_train, k, m->n_classes, labels, scores, flag, nb_ind, nb_dist);
+        kern<<<(unsigned)blocks, kKnnThreads, smem, st>>>(static_cast<const double *>(x), n, m->d, m->d_fit, m->d_y, m->n_train,
+                                                          call.k, m->n_classes, call.labels, call.scores, flag, call.ind, call.dist);
     }
     TCSDN_CUDA(cudaGetLastError());
     return TCSDN_OK;
-}
-
-int launch_knn_exact(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, double *scores,
-                     int32_t *flag, cudaStream_t st) {
-    return launch_exact(m, x, n, dtype, predict_out(m), m->k, labels, scores, nullptr, nullptr, flag, st);
-}
-
-int launch_knn_exact_kneighbors(tcsdn_model *m, const void *x, int64_t n, int dtype, int nn, int64_t *ind, double *dist,
-                                int32_t *flag, cudaStream_t st) {
-    return launch_exact(m, x, n, dtype, KnnOut::Neighbors, nn, nullptr, nullptr, ind, dist, flag, st);
 }
 
 // The tensor-core engine's tie rows (dist_engine.cu): a few rows per ten thousand whose label depends on which of several
@@ -210,9 +193,8 @@ static auto tie_kernel(KnnOut out) {
                                          : knn_tie_kernel<T, KnnOut::Vote>;
 }
 
-static int launch_marked(tcsdn_model *m, const void *x, int64_t n, int dtype, KnnOut out, int k, int32_t *labels, double *scores,
-                         int64_t *nb_ind, double *nb_dist, const int32_t *list, const int *count, unsigned long long *total,
-                         cudaStream_t st) {
+int launch_knn_marked(tcsdn_model *m, const void *x, int64_t n, int dtype, const KnnCall &call, const int32_t *list,
+                      const int *count, unsigned long long *total, cudaStream_t st) {
     if (n == 0) return TCSDN_OK;
     if (m->d > kTieMaxD) { set_error("knn tie kernel: more than %d features", kTieMaxD); return TCSDN_EINVAL; }
     int64_t blocks = (n + 7) / 8;                     // eight rows (warps) per block
@@ -220,26 +202,16 @@ static int launch_marked(tcsdn_model *m, const void *x, int64_t n, int dtype, Kn
     if (blocks > cap) blocks = cap;
     m->stats[0] += 1;
     if (dtype == TCSDN_F32) {
-        auto kern = tie_kernel<float>(out);
-        kern<<<(unsigned)blocks, 256, 0, st>>>(static_cast<const float *>(x), m->d, m->d_fit, m->d_y, m->n_train, k, m->n_classes,
-                                               labels, scores, list, count, total, nb_ind, nb_dist);
+        auto kern = tie_kernel<float>(call.out);
+        kern<<<(unsigned)blocks, 256, 0, st>>>(static_cast<const float *>(x), m->d, m->d_fit, m->d_y, m->n_train, call.k,
+                                               m->n_classes, call.labels, call.scores, list, count, total, call.ind, call.dist);
     } else {
-        auto kern = tie_kernel<double>(out);
-        kern<<<(unsigned)blocks, 256, 0, st>>>(static_cast<const double *>(x), m->d, m->d_fit, m->d_y, m->n_train, k, m->n_classes,
-                                               labels, scores, list, count, total, nb_ind, nb_dist);
+        auto kern = tie_kernel<double>(call.out);
+        kern<<<(unsigned)blocks, 256, 0, st>>>(static_cast<const double *>(x), m->d, m->d_fit, m->d_y, m->n_train, call.k,
+                                               m->n_classes, call.labels, call.scores, list, count, total, call.ind, call.dist);
     }
     TCSDN_CUDA(cudaGetLastError());
     return TCSDN_OK;
-}
-
-int launch_knn_marked(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, double *scores,
-                      const int32_t *list, const int *count, unsigned long long *total, cudaStream_t st) {
-    return launch_marked(m, x, n, dtype, predict_out(m), m->k, labels, scores, nullptr, nullptr, list, count, total, st);
-}
-
-int launch_knn_marked_kneighbors(tcsdn_model *m, const void *x, int64_t n, int dtype, int nn, int64_t *ind, double *dist,
-                                 const int32_t *list, const int *count, unsigned long long *total, cudaStream_t st) {
-    return launch_marked(m, x, n, dtype, KnnOut::Neighbors, nn, nullptr, nullptr, ind, dist, list, count, total, st);
 }
 
 }  // namespace tcsdn

@@ -165,47 +165,17 @@ class _Base:
         """-> (indices, scores or None); numpy in -> numpy out, CUDA tensor in -> CUDA tensors out.
         `out`: optional preallocated int32 index buffer (same kind/location as X), e.g. for CUDA graphs."""
         self._check_fitted()
-        lib = _lib.load()
-        if _is_torch_cuda(X):
-            import torch
-            if X.dim() != 2:
-                raise ValueError(f"Expected 2D array, got {X.dim()}D tensor instead")
-            if X.dtype not in (torch.float32, torch.float64):
-                X = X.to(torch.float64)
-            X = X.contiguous()
-            n, d = X.shape
-            if out is not None:
+        X, n, d, dt, loc = _rows(X)
+        if out is not None:
+            if loc == _lib.DEVICE:
+                import torch
                 if not (_is_torch_cuda(out) and out.dtype == torch.int32 and out.numel() == n and out.is_contiguous()):
                     raise ValueError("out must be a contiguous CUDA int32 tensor with one element per row")
-                labels = out
-            else:
-                labels = torch.empty(n, dtype=torch.int32, device=X.device)
-            scores = torch.empty((n, self._score_cols), dtype=torch.float64, device=X.device) if want_scores else None
-            with torch.cuda.device(X.device):
-                st = torch.cuda.current_stream().cuda_stream
-                _lib.check(lib.tcsdn_predict(self._handle, X.data_ptr(), n, d,
-                                             _lib.F32 if X.dtype == torch.float32 else _lib.F64, _lib.DEVICE,
-                                             labels.data_ptr(), scores.data_ptr() if want_scores else None, st))
-            return labels, scores
-        A = X if isinstance(X, np.ndarray) else np.asarray(X)
-        if A.ndim != 2:
-            raise ValueError(f"Expected 2D array, got {A.ndim}D array instead:\narray={A!r}.\nReshape your data "
-                             "either using array.reshape(-1, 1) if your data has a single feature or "
-                             "array.reshape(1, -1) if it contains a single sample.")
-        if A.dtype not in (np.float32, np.float64):
-            A = A.astype(np.float64)  # what validate_data does with ints / Python floats
-        A = np.ascontiguousarray(A)
-        n, d = A.shape
-        if out is not None:
-            if not (isinstance(out, np.ndarray) and out.dtype == np.int32 and out.shape == (n,) and out.flags.c_contiguous):
+            elif not (isinstance(out, np.ndarray) and out.dtype == np.int32 and out.shape == (n,) and out.flags.c_contiguous):
                 raise ValueError("out must be a contiguous int32 array with one element per row")
-            labels = out
-        else:
-            labels = np.empty(n, np.int32)
-        scores = np.empty((n, self._score_cols), np.float64) if want_scores else None
-        _lib.check(lib.tcsdn_predict(self._handle, _lib.ptr(A), n, d, _lib.F32 if A.dtype == np.float32 else _lib.F64,
-                                     _lib.HOST, _lib.ptr(labels), _lib.ptr(scores) if want_scores else None, None))
-        return labels, scores
+        lib = _lib.load()
+        return _call(X, loc, [((n,), np.int32) if out is None else out, ((n, self._score_cols), np.float64) if want_scores else None],
+                     lambda x, o, st: lib.tcsdn_predict(self._handle, x, n, d, dt, loc, o[0], o[1], st))
 
     def sync_check(self):
         """After CUDA-tensor predicts: wait for the current stream and raise ValueError on NaN/inf input."""
@@ -253,6 +223,45 @@ class _Base:
 
 def _p(a, t):
     return a.ctypes.data_as(t)
+
+
+def _rows(X):
+    """-> (rows, n, d, dtype code, loc code) for a query: a contiguous float32/float64 CUDA tensor or numpy array (other
+    dtypes are widened to float64, what validate_data does with ints / Python floats)."""
+    if _is_torch_cuda(X):
+        import torch
+        if X.dim() != 2:
+            raise ValueError(f"Expected 2D array, got {X.dim()}D tensor instead")
+        if X.dtype not in (torch.float32, torch.float64):
+            X = X.to(torch.float64)
+        X = X.contiguous()
+        return X, X.shape[0], X.shape[1], _lib.F32 if X.dtype == torch.float32 else _lib.F64, _lib.DEVICE
+    A = X if isinstance(X, np.ndarray) else np.asarray(X)
+    if A.ndim != 2:
+        raise ValueError(f"Expected 2D array, got {A.ndim}D array instead:\narray={A!r}.\nReshape your data "
+                         "either using array.reshape(-1, 1) if your data has a single feature or "
+                         "array.reshape(1, -1) if it contains a single sample.")
+    if A.dtype not in (np.float32, np.float64):
+        A = A.astype(np.float64)
+    A = np.ascontiguousarray(A)
+    return A, A.shape[0], A.shape[1], _lib.F32 if A.dtype == np.float32 else _lib.F64, _lib.HOST
+
+
+def _call(X, loc, outs, fn):
+    """-> the outputs of ``fn(x, out_pointers, stream)`` on the rows X (from _rows).  Each entry of ``outs`` is a
+    ``(shape, numpy dtype)`` allocated where X lives, a preallocated buffer, or None (no output, a null pointer).  CUDA rows
+    run on the current stream of X's device; host rows pass no stream."""
+    if loc == _lib.DEVICE:
+        import torch
+        outs = [torch.empty(o[0], dtype=getattr(torch, np.dtype(o[1]).name), device=X.device) if isinstance(o, tuple) else o
+                for o in outs]
+        with torch.cuda.device(X.device):
+            st = torch.cuda.current_stream().cuda_stream
+            _lib.check(fn(X.data_ptr(), [None if o is None else o.data_ptr() for o in outs], st))
+        return tuple(outs)
+    outs = [np.empty(*o) if isinstance(o, tuple) else o for o in outs]
+    _lib.check(fn(_lib.ptr(X), [None if o is None else _lib.ptr(o) for o in outs], None))
+    return tuple(outs)
 
 
 class LogisticRegression(_Base):
@@ -488,7 +497,7 @@ class KNeighborsClassifier(_Base):
         if query_is_train:
             X = np.ascontiguousarray(self._spec["fit_X"], np.float64)
             n_neighbors += 1                         # the row itself comes back too and is removed below
-        X, n, d, dt, loc = self._query_rows(X)
+        X, n, d, dt, loc = _rows(X)
         if d != self.n_features_in_:
             raise ValueError(f"X has {d} features, but {type(self).__name__} is expecting {self.n_features_in_} features as input")
         if n_neighbors > self.n_samples_fit_:
@@ -503,19 +512,10 @@ class KNeighborsClassifier(_Base):
             raise ValueError(f"kneighbors keeps at most 64 neighbours per row (with X=None: 63), got n_neighbors = "
                              f"{n_neighbors - 1 if query_is_train else n_neighbors}")
         lib = _lib.load()
+        ind, dist = _call(X, loc, [((n, n_neighbors), np.int64), ((n, n_neighbors), np.float64) if return_distance else None],
+                          lambda x, o, st: lib.tcsdn_knn_kneighbors(self._handle, x, n, d, dt, loc, n_neighbors, o[0], o[1], st))
         if loc == _lib.DEVICE:
-            import torch
-            ind = torch.empty((n, n_neighbors), dtype=torch.int64, device=X.device)
-            dist = torch.empty((n, n_neighbors), dtype=torch.float64, device=X.device) if return_distance else None
-            with torch.cuda.device(X.device):
-                st = torch.cuda.current_stream().cuda_stream
-                _lib.check(lib.tcsdn_knn_kneighbors(self._handle, X.data_ptr(), n, d, dt, loc, n_neighbors, ind.data_ptr(),
-                                                    dist.data_ptr() if return_distance else None, st))
             return (dist, ind) if return_distance else ind
-        ind = np.empty((n, n_neighbors), np.int64)
-        dist = np.empty((n, n_neighbors), np.float64) if return_distance else None
-        _lib.check(lib.tcsdn_knn_kneighbors(self._handle, _lib.ptr(X), n, d, dt, loc, n_neighbors, _lib.ptr(ind),
-                                            _lib.ptr(dist) if return_distance else None, None))
         if query_is_train:
             # sk:neighbors/_base.py:930-956: drop each row's own index; where more duplicates than neighbours push it out
             # of the n_neighbors + 1 kept rows, drop the first column instead
@@ -525,26 +525,6 @@ class KNeighborsClassifier(_Base):
             if return_distance:
                 dist = dist[keep].reshape(n, n_neighbors - 1)
         return (dist, ind) if return_distance else ind
-
-    @staticmethod
-    def _query_rows(X):
-        """-> (rows, n, d, dtype code, loc code) for a query: a contiguous float32/float64 CUDA tensor or numpy array
-        (other dtypes are widened to float64, as predict does)."""
-        if _is_torch_cuda(X):
-            import torch
-            if X.dim() != 2:
-                raise ValueError(f"Expected 2D array, got {X.dim()}D tensor instead")
-            if X.dtype not in (torch.float32, torch.float64):
-                X = X.to(torch.float64)
-            X = X.contiguous()
-            return X, X.shape[0], X.shape[1], _lib.F32 if X.dtype == torch.float32 else _lib.F64, _lib.DEVICE
-        A = X if isinstance(X, np.ndarray) else np.asarray(X)
-        if A.ndim != 2:
-            raise ValueError(f"Expected 2D array, got {A.ndim}D array instead")
-        if A.dtype not in (np.float32, np.float64):
-            A = A.astype(np.float64)
-        A = np.ascontiguousarray(A)
-        return A, A.shape[0], A.shape[1], _lib.F32 if A.dtype == np.float32 else _lib.F64, _lib.HOST
 
 
 class SVC(_Base):
