@@ -62,7 +62,12 @@ enum { /* tcsdn_set_option() keys */
                                     from the fp64 kernel),
                                   3 engine in audit mode, tests only (knn: filter off; svc: scores_out receives the engine's
                                     uncorrected decision values; both: tensor-core error statistic in stats[5]),
-                                  4 svc engine, tests only: scores_out receives the certificate's per-pair error bounds */
+                                  4 svc engine, tests only: scores_out receives the certificate's per-pair error bounds.
+                                  SVC handles of the other kernels (tcsdn_svc_create_kernel) have no tensor-core engine:
+                                  linear -- 2, 3 and 4 apply to the collapsed label path (2 forces it for label-only calls,
+                                    TCSDN_EINVAL when the model's shape has none; 3 / 4 write its raw decision values / its
+                                    per-pair bounds to scores_out); poly, sigmoid -- 2, 3 and 4 return TCSDN_EINVAL;
+                                  1 keeps every kernel on the fp64 kernel */
     TCSDN_OPT_CHUNK_ROWS = 2,  /* host-pointer pipeline chunk (rows); 0 = default */
     TCSDN_OPT_CHECK_FINITE = 3, /* 1 (default): fail with TCSDN_ENONFINITE on NaN/inf input */
     /* measurement knobs (bench.py --set-option sweeps them) */
@@ -119,6 +124,25 @@ int tcsdn_svc_create(const double *sv, const double *dual_coef, const double *in
                      const int32_t *n_support, int32_t n_sv, int32_t d, int32_t n_classes,
                      double gamma, tcsdn_model_t **out);
 
+enum { /* tcsdn_svc_create_kernel() kernel: libsvm's numbering */
+    TCSDN_SVC_LINEAR = 0, TCSDN_SVC_POLY = 1, TCSDN_SVC_RBF = 2, TCSDN_SVC_SIGMOID = 3
+};
+
+/* SVC(kernel='linear' | 'poly' | 'rbf' | 'sigmoid'): as tcsdn_svc_create, plus the kernel and its parameters
+ * (sk:svm/src/libsvm/svm.cpp:452-515): linear K = dot(x, sv); poly K = powi(gamma * dot(x, sv) + coef0, degree);
+ * rbf K = exp(-gamma ||x - sv||^2); sigmoid K = tanh(gamma * dot(x, sv) + coef0).  dot is an fma chain in feature order,
+ * powi libsvm's square-and-multiply loop (degree 0 gives 1.0).  TCSDN_SVC_RBF is tcsdn_svc_create (gamma > 0, coef0 and
+ * degree ignored).  The other kernels: gamma finite and >= 0 (sklearn allows gamma=0.0), coef0 finite, poly degree >= 0;
+ * TCSDN_EINVAL otherwise and for any other kernel value.  Decision values, and the labels of poly and sigmoid models, come
+ * from the fp64 kernel.  Label-only predicts on linear models with n_classes <= 8 and n_features <= 16 take the collapsed
+ * path: per pair p the weights W_p = sum_s coef_ps sv_s are formed at create time, a row costs P x d fp64 FMAs, and a
+ * per-pair error bound certifies each row's vote against the fp64 kernel's; rows it cannot certify are re-run by the fp64
+ * kernel in the same call (counted in stats[6]), so labels are the fp64 kernel's on every row.  Rows of both paths count in
+ * stats[2]. */
+int tcsdn_svc_create_kernel(const double *sv, const double *dual_coef, const double *intercept,
+                            const int32_t *n_support, int32_t n_sv, int32_t d, int32_t n_classes,
+                            int32_t kernel, double gamma, double coef0, int32_t degree, tcsdn_model_t **out);
+
 /* RandomForestClassifier: trees concatenated; tree t owns nodes [tree_offsets[t], tree_offsets[t+1]);
  * left/right are node indices local to the tree (-1 = leaf); value [n_nodes][n_classes] are the
  * per-node class fractions DecisionTreeClassifier.predict_proba returns.
@@ -141,7 +165,7 @@ int tcsdn_set_option(tcsdn_model_t *m, int32_t key, int64_t value);
  * engine, [2] rows through the fp64 CUDA-core kernels, [3] exact fp64 re-evaluations of the knn filter (cumulative
  * since create), [4] knn engine: reference tiles multiplied per 512-row pass, times 1000 (cumulative average), [5] largest observed |tensor-core value - exact| / (the error model's denominator), times 2^40
  * (cumulative, audit mode), [6] rows a certified fast path could not decide and handed to the fp64 definition
- * (GaussianNB fp32 pre-pass, svc engine; cumulative since create), [7] knn engine: rows whose label depended on a tie at
+ * (GaussianNB fp32 pre-pass, svc engine, linear svc collapsed path; cumulative since create), [7] knn engine: rows whose label depended on a tie at
  * the k-th distance and were re-run by the index-order fp64 kernel (cumulative).  out has 8 slots.  Reading the
  * device-side counters synchronises the device.  Concurrent predicts on one handle add up in [0..2]. */
 int tcsdn_model_stats(const tcsdn_model_t *m, int64_t *out);

@@ -17,6 +17,8 @@ OPT_ENGINE, OPT_CHUNK_ROWS, OPT_CHECK_FINITE = 1, 2, 3
 OPT_SCORER_SHAPE, OPT_FOREST_SHAPE, OPT_FOREST_SORT, OPT_KNN_FLUSH_TILES, OPT_KNN_PRUNE = 4, 5, 6, 7, 8
 FLOW_STATE = 19
 KNN_UNIFORM, KNN_DISTANCE = 0, 1
+SVC_LINEAR, SVC_POLY, SVC_RBF, SVC_SIGMOID = 0, 1, 2, 3
+SVC_KERNELS = {"linear": SVC_LINEAR, "poly": SVC_POLY, "rbf": SVC_RBF, "sigmoid": SVC_SIGMOID}
 COMM_ID_BYTES = 128
 
 _vp = C.c_void_p
@@ -39,6 +41,8 @@ SIGNATURES = {
                                             C.POINTER(_vp)]),
     "tcsdn_svc_create": (C.c_int, [_f64p, _f64p, _f64p, _i32p, C.c_int32, C.c_int32, C.c_int32, C.c_double,
                                    C.POINTER(_vp)]),
+    "tcsdn_svc_create_kernel": (C.c_int, [_f64p, _f64p, _f64p, _i32p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_double,
+                                          C.c_double, C.c_int32, C.POINTER(_vp)]),
     "tcsdn_forest_create": (C.c_int, [_i64p, _i32p, _i32p, _i32p, _f64p, _f64p, C.c_int32, C.c_int32, C.c_int32,
                                       C.POINTER(_vp)]),
     "tcsdn_destroy": (None, [_vp]),

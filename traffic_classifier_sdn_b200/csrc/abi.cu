@@ -141,7 +141,13 @@ static int run_device(tcsdn_model *m, const void *x, int64_t n, int dtype, int32
             // decision values are always the fp64 kernel's (the engine certifies LABELS; its fp32 sums cannot meet a
             // 1e-5 absolute bound on decision values, see dist_engine.cu)
             if (m->opt_engine != 1 && engine_usable(m, n, scores != nullptr)) return launch_svc_engine(m, x, n, dtype, labels, scores, flag, st);
-            if (m->opt_engine >= 2 && !scores) { set_error("tensor-core engine forced but not usable for this model/batch"); return TCSDN_EINVAL; }
+            // linear kernel: the collapsed label path (svc.cu), certified against the fp64 kernel like the engine
+            if (m->opt_engine != 1 && svc_linear_usable(m, scores != nullptr)) return launch_svc_linear(m, x, n, dtype, labels, scores, flag, st);
+            if (m->opt_engine >= 2 && !scores) {
+                set_error(m->svc_kernel == TCSDN_SVC_LINEAR ? "collapsed linear path forced but not usable for this model (n_classes <= 8, n_features <= 16)"
+                                                            : "tensor-core engine forced but not usable for this model/batch");
+                return TCSDN_EINVAL;
+            }
             return launch_svc_exact(m, x, n, dtype, labels, scores, flag, st);
     }
     set_error("corrupt model handle");
@@ -439,13 +445,28 @@ int tcsdn_knn_create_weighted(const double *fit_x, const int32_t *y, int64_t n_t
 
 int tcsdn_svc_create(const double *sv, const double *dual_coef, const double *intercept, const int32_t *n_support,
                      int32_t n_sv, int32_t d, int32_t n_classes, double gamma, tcsdn_model_t **out) {
+    return tcsdn_svc_create_kernel(sv, dual_coef, intercept, n_support, n_sv, d, n_classes, TCSDN_SVC_RBF, gamma, 0.0, 3, out);
+}
+
+int tcsdn_svc_create_kernel(const double *sv, const double *dual_coef, const double *intercept, const int32_t *n_support,
+                            int32_t n_sv, int32_t d, int32_t n_classes, int32_t kernel, double gamma, double coef0, int32_t degree,
+                            tcsdn_model_t **out) {
     if (!out) { set_error("out handle pointer is NULL"); return TCSDN_EINVAL; }
     *out = nullptr;
     if (!sv || !dual_coef || !intercept || !n_support || n_sv < 1 || n_classes < 2 || n_classes > 16) {
         set_error("svc: bad arguments (2 <= n_classes <= 16)");
         return TCSDN_EINVAL;
     }
-    if (!(gamma > 0.0) || !std::isfinite(gamma)) { set_error("svc: gamma must be finite and > 0"); return TCSDN_EINVAL; }
+    if (kernel == TCSDN_SVC_RBF) {
+        if (!(gamma > 0.0) || !std::isfinite(gamma)) { set_error("svc: gamma must be finite and > 0"); return TCSDN_EINVAL; }
+    } else if (kernel == TCSDN_SVC_LINEAR || kernel == TCSDN_SVC_POLY || kernel == TCSDN_SVC_SIGMOID) {
+        if (!(gamma >= 0.0) || !std::isfinite(gamma)) { set_error("svc: gamma must be finite and >= 0"); return TCSDN_EINVAL; }
+        if (!std::isfinite(coef0)) { set_error("svc: coef0 must be finite"); return TCSDN_EINVAL; }
+        if (kernel == TCSDN_SVC_POLY && degree < 0) { set_error("svc: degree must be >= 0, got %d", degree); return TCSDN_EINVAL; }
+    } else {
+        set_error("svc: kernel must be TCSDN_SVC_LINEAR, TCSDN_SVC_POLY, TCSDN_SVC_RBF or TCSDN_SVC_SIGMOID, got %d", kernel);
+        return TCSDN_EINVAL;
+    }
     const int P = n_classes * (n_classes - 1) / 2;
     std::vector<int32_t> start(n_classes + 1, 0);
     for (int i = 0; i < n_classes; ++i) {
@@ -460,13 +481,16 @@ int tcsdn_svc_create(const double *sv, const double *dual_coef, const double *in
     tcsdn_model *m;
     TCSDN_TRY(model_base(&m, TCSDN_KIND_SVC, d, n_classes, P));
     m->n_sv = n_sv; m->gamma = gamma;
+    if (kernel != TCSDN_SVC_RBF) { m->svc_kernel = kernel; m->coef0 = coef0; m->degree = degree; }
     std::vector<double> rho(P);
     for (int p = 0; p < P; ++p) rho[p] = -intercept[p];  // sk:svm/src/libsvm/libsvm_helper.c:171
     int r = upload(&m->d_sv, sv, (size_t)n_sv * d);
     if (r == TCSDN_OK) r = upload(&m->d_coef, dual_coef, (size_t)(n_classes - 1) * n_sv);
     if (r == TCSDN_OK) r = upload(&m->d_rho, rho.data(), rho.size());
     if (r == TCSDN_OK) r = upload(&m->d_start, start.data(), start.size());
-    if (r == TCSDN_OK) r = svc_engine_create(m);
+    // the tensor-core engine's certificate is the rbf kernel's; a linear model gets the collapsed label path instead
+    if (r == TCSDN_OK && kernel == TCSDN_SVC_RBF) r = svc_engine_create(m);
+    if (r == TCSDN_OK && kernel == TCSDN_SVC_LINEAR) r = svc_linear_create(m, sv, dual_coef, rho.data(), start.data());
     if (r != TCSDN_OK) { tcsdn_destroy(m); return r; }
     *out = m;
     return TCSDN_OK;
@@ -499,7 +523,7 @@ void tcsdn_destroy(tcsdn_model_t *m) {
     for (Workspace *w : m->pool) free_workspace(w);
     cudaFree(m->d_a); cudaFree(m->d_b); cudaFree(m->d_c);
     cudaFree(m->d_fit); cudaFree(m->d_y);
-    cudaFree(m->d_sv); cudaFree(m->d_coef); cudaFree(m->d_rho); cudaFree(m->d_start);
+    cudaFree(m->d_sv); cudaFree(m->d_coef); cudaFree(m->d_rho); cudaFree(m->d_start); cudaFree(m->d_lin);
     cudaFree(m->d_nodes); cudaFree(m->d_tree_base); cudaFree(m->d_group_begin); cudaFree(m->d_leaf_val);
     cudaFree(m->d_flag);
     cudaFree(m->d_refined);
@@ -516,6 +540,10 @@ int tcsdn_set_option(tcsdn_model_t *m, int32_t key, int64_t value) {
     switch (key) {
         case TCSDN_OPT_ENGINE:
             if (value < 0 || value > 4) { set_error("engine option must be 0..4"); return TCSDN_EINVAL; }
+            if (value >= 2 && m->kind == TCSDN_KIND_SVC && (m->svc_kernel == TCSDN_SVC_POLY || m->svc_kernel == TCSDN_SVC_SIGMOID)) {
+                set_error("engine options 2..4: poly and sigmoid SVC models have no fast path (the fp64 kernel runs every call)");
+                return TCSDN_EINVAL;
+            }
             m->opt_engine = value; return TCSDN_OK;
         case TCSDN_OPT_CHUNK_ROWS:
             if (value < 0) { set_error("chunk rows must be >= 0"); return TCSDN_EINVAL; }

@@ -292,6 +292,10 @@ struct tcsdn_model {
     int32_t *d_start = nullptr;  // [C+1] class starts
     int n_sv = 0;
     double gamma = 0.0;
+    int svc_kernel = TCSDN_SVC_RBF;   // TCSDN_SVC_LINEAR / POLY / RBF / SIGMOID
+    double coef0 = 0.0;
+    int degree = 3;
+    double *d_lin = nullptr;     // linear kernel, C <= 8, d <= 16: the collapsed path's parameters (svc.cu), else null
 
     // ---- forest
     uint2 *d_nodes = nullptr;        // packed preorder nodes, all trees
@@ -306,7 +310,7 @@ struct tcsdn_model {
 
     // ---- per-handle misc
     int32_t *d_flag = nullptr;       // device error flag (non-finite input)
-    unsigned long long *d_refined = nullptr;   // GaussianNB: rows the fp32 pre-pass could not certify (re-run in fp64)
+    unsigned long long *d_refined = nullptr;   // GaussianNB / linear SVC: rows the certified fast path could not decide (re-run in fp64)
     std::mutex mu;
     std::vector<tcsdn::Workspace *> pool;
     void *engine = nullptr;          // tensor-core engine state (dist_engine.cu), may be null
@@ -363,6 +367,12 @@ void engine_read_stats(const tcsdn_model *m, int64_t *out8);
 // `counter` (device) receives the number of such rows
 int launch_svc_marked(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, unsigned long long *counter,
                       cudaStream_t st);
+// svc.cu, linear kernel: the collapsed label path (certified; uncertified rows re-run by launch_svc_marked in the same call),
+// its parameters built at create time (nothing for shapes it does not take), and whether it takes a call
+int launch_svc_linear(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, double *scores, int32_t *flag,
+                      cudaStream_t st);
+int svc_linear_create(tcsdn_model *m, const double *sv, const double *coef, const double *rho, const int32_t *start);
+bool svc_linear_usable(const tcsdn_model *m, bool want_scores);
 int launch_knn_engine(tcsdn_model *m, const void *x, int64_t n, int dtype, const KnnCall &call, int32_t *flag, cudaStream_t st);
 int launch_svc_engine(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, double *scores,
                       int32_t *flag, cudaStream_t st);

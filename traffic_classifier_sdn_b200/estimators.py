@@ -528,7 +528,7 @@ class KNeighborsClassifier(_Base):
 
 
 class SVC(_Base):
-    """sk:svm/src/libsvm/svm.cpp:461-478,2846-2904 -- RBF kernel values, one-vs-one sums, vote."""
+    """sk:svm/src/libsvm/svm.cpp:452-515,2846-2904 -- kernel values (linear, poly, rbf, sigmoid), one-vs-one sums, vote."""
     _kind = "svc"
 
     def _sk_estimator(self):
@@ -543,9 +543,38 @@ class SVC(_Base):
         self.support_vectors_, self.n_support_, self._gamma = sv, nsup, float(spec["gamma"])
         self.decision_function_shape = spec.get("decision_function_shape", "ovr")
         self.break_ties = bool(spec.get("break_ties", False))
-        _lib.check(lib.tcsdn_svc_create(_p(sv, _lib._f64p), _p(dual, _lib._f64p), _p(icpt, _lib._f64p),
-                                        _p(nsup, _lib._i32p), sv.shape[0], sv.shape[1], len(nsup),
-                                        float(spec["gamma"]), C.byref(h)))
+        self.kernel = modelio.svc_kernel(spec.get("kernel", "rbf"))
+        self.coef0, self.degree = float(spec.get("coef0", 0.0)), int(spec.get("degree", 3))
+        if self.kernel == "rbf":
+            _lib.check(lib.tcsdn_svc_create(_p(sv, _lib._f64p), _p(dual, _lib._f64p), _p(icpt, _lib._f64p),
+                                            _p(nsup, _lib._i32p), sv.shape[0], sv.shape[1], len(nsup),
+                                            float(spec["gamma"]), C.byref(h)))
+        else:
+            _lib.check(lib.tcsdn_svc_create_kernel(_p(sv, _lib._f64p), _p(dual, _lib._f64p), _p(icpt, _lib._f64p),
+                                                   _p(nsup, _lib._i32p), sv.shape[0], sv.shape[1], len(nsup),
+                                                   _lib.SVC_KERNELS[self.kernel], float(spec["gamma"]), self.coef0,
+                                                   self.degree, C.byref(h)))
+
+    @property
+    def coef_(self):
+        """Primal weights of a linear model, one row per class pair (sk:svm/_base.py:_get_coef, _one_vs_one_coef): from the
+        public dual coefficients, which are libsvm's negated for two classes.  Read-only, as in sklearn."""
+        self._check_fitted()
+        if self.kernel != "linear":
+            raise AttributeError("coef_ is only available when using a linear kernel")
+        sv, dual = self.support_vectors_, np.asarray(self._spec["dual_coef"], np.float64)
+        if dual.shape[0] == 1:
+            coef = (-dual) @ sv
+        else:
+            loc = np.cumsum(np.hstack([[0], self.n_support_]))
+            rows = []
+            for c1 in range(dual.shape[0] + 1):
+                for c2 in range(c1 + 1, dual.shape[0] + 1):
+                    rows.append(dual[c2 - 1, loc[c1]:loc[c1 + 1]] @ sv[loc[c1]:loc[c1 + 1]] +
+                                dual[c1, loc[c2]:loc[c2 + 1]] @ sv[loc[c2]:loc[c2 + 1]])
+            coef = np.vstack(rows)
+        coef.flags.writeable = False
+        return coef
 
     def _ovo(self, X):
         return self._scores(X)

@@ -21,7 +21,8 @@ kmeans     centers [k,d]
 knn        fit_X [n_t,d] f64, y [n_t] int32 (class index), k, classes, weights ("uniform" or
            "distance"; a spec without the key is uniform)
 svc        sv [nSV,d], dual_coef [C-1,nSV], intercept [P], n_support [C] int32,
-           gamma, classes, decision_function_shape, break_ties
+           gamma, classes, decision_function_shape, break_ties, kernel ("linear", "poly", "rbf" or
+           "sigmoid"; a spec without the key is rbf), coef0, degree
 forest     tree_offsets [T+1] int64, left/right/feature int32 [N], threshold f64 [N],
            value [N,C] f64 (per-node class fractions), classes
 =========  ==========================================================================
@@ -35,7 +36,7 @@ from typing import Any, Dict
 import numpy as np
 
 __all__ = ["load_reference_pickle", "spec_from_estimator", "spec_from_pickle_bytes",
-           "knn_weights", "MODEL_FILES", "SpecError"]
+           "knn_weights", "svc_kernel", "MODEL_FILES", "SpecError"]
 
 # argv word -> pickle file, as dispatched at reference traffic_classifier.py:229-240
 MODEL_FILES = {
@@ -157,6 +158,16 @@ def knn_weights(w) -> str:
     raise SpecError(f"weights must be 'uniform' or 'distance', got {w!r}")
 
 
+def svc_kernel(k) -> str:
+    """SVC's ``kernel`` as a spec value: one of libsvm's four built-in kernels.  'precomputed' and callables need the
+    training rows at predict time and are refused."""
+    if callable(k):
+        raise SpecError("callable kernels are not implemented (kernel must be 'linear', 'poly', 'rbf' or 'sigmoid')")
+    if isinstance(k, str) and k in ("linear", "poly", "rbf", "sigmoid"):
+        return k
+    raise SpecError(f"kernel must be 'linear', 'poly', 'rbf' or 'sigmoid', got {k!r}")
+
+
 def _spec_from_attrs(name: str, o) -> Dict[str, Any]:
     if name == "LogisticRegression":
         coef = _f64(o.coef_)
@@ -190,8 +201,7 @@ def _spec_from_attrs(name: str, o) -> Dict[str, Any]:
         return dict(kind="knn", fit_X=fx, y=np.ascontiguousarray(y, dtype=np.int32),
                     k=int(o.n_neighbors), classes=_classes(o), n_features=fx.shape[1], weights=weights)
     if name == "SVC":
-        if o.kernel != "rbf":
-            raise SpecError("only kernel='rbf' is implemented")
+        kernel = svc_kernel(getattr(o, "kernel", "rbf"))   # pickles without the attribute are rbf models
         if getattr(o, "_sparse", False):
             raise SpecError("sparse SVC is not supported")
         sv = _f64(o.support_vectors_)
@@ -205,7 +215,8 @@ def _spec_from_attrs(name: str, o) -> Dict[str, Any]:
         return dict(kind="svc", sv=sv, dual_coef=dual, intercept=icpt, n_support=np.ascontiguousarray(nsup),
                     gamma=float(o._gamma), classes=cls, n_features=sv.shape[1],
                     decision_function_shape=str(o.decision_function_shape),
-                    break_ties=bool(getattr(o, "break_ties", False)), n_classes=C)
+                    break_ties=bool(getattr(o, "break_ties", False)), n_classes=C, kernel=kernel,
+                    coef0=float(getattr(o, "coef0", 0.0)), degree=int(getattr(o, "degree", 3)))
     if name == "RandomForestClassifier":
         cls = _classes(o)
         if cls is None or (len(cls) and isinstance(cls[0], np.ndarray)):
