@@ -117,6 +117,24 @@ enum { TCSDN_KNN_UNIFORM = 0, TCSDN_KNN_DISTANCE = 1 }; /* tcsdn_knn_create_weig
 int tcsdn_knn_create_weighted(const double *fit_x, const int32_t *y, int64_t n_train, int32_t d,
                               int32_t n_classes, int32_t k, int32_t weights, tcsdn_model_t **out);
 
+enum { /* tcsdn_knn_create_metric() metric */
+    TCSDN_KNN_EUCLIDEAN = 0, TCSDN_KNN_MANHATTAN = 1, TCSDN_KNN_CHEBYSHEV = 2
+};
+
+/* KNeighborsClassifier(metric='euclidean' | 'manhattan' | 'chebyshev'): as tcsdn_knn_create_weighted, with the metric
+ * (TCSDN_KNN_EUCLIDEAN is tcsdn_knn_create_weighted).  Per pair the library ranks by rdist, fp64, features in order from
+ * 0.0, float32 rows widened first: euclidean sum (x_f - t_f)^2 (the distance is its correctly rounded sqrt), manhattan
+ * sum |x_f - t_f| (sequential adds, sk:metrics/_dist_metrics.pyx.tp ManhattanDistance), chebyshev max |x_f - t_f|
+ * (ChebyshevDistance); for the last two the distance is rdist itself, so neighbours, distances, labels and scores equal
+ * scikit-learn's brute force bit for bit (equal distances in (distance, training index) order, as for euclidean).
+ * Distance weights are 1 / distance.  Any other metric value returns TCSDN_EINVAL before any device work.
+ * Manhattan and chebyshev handles with n_features <= 12 and k <= 32 run batches of 1024 rows or more on a pruned CUDA-core
+ * kernel over the same spatial index as the euclidean engine (rows through it count in stats[1], "engine rows"); the
+ * rest on the fp64 kernel.  TCSDN_OPT_ENGINE: 1 forces the fp64 kernel, 2 forces the pruned kernel (TCSDN_EINVAL when it
+ * is not usable), 3 and 4 return TCSDN_EINVAL.  TCSDN_OPT_KNN_PRUNE = 1 makes the pruned kernel visit every tile. */
+int tcsdn_knn_create_metric(const double *fit_x, const int32_t *y, int64_t n_train, int32_t d,
+                            int32_t n_classes, int32_t k, int32_t weights, int32_t metric, tcsdn_model_t **out);
+
 /* SVC(kernel='rbf'): support_vectors_ [n_sv][d] grouped by class, _dual_coef_ [n_classes-1][n_sv],
  * _intercept_ [n_classes*(n_classes-1)/2], _n_support [n_classes], _gamma.
  * sk:svm/src/libsvm/svm.cpp:461-478,2846-2904; sk:svm/src/libsvm/libsvm_helper.c:171. */
@@ -156,14 +174,16 @@ void tcsdn_destroy(tcsdn_model_t *m);
 int tcsdn_model_kind(const tcsdn_model_t *m);
 int tcsdn_model_n_features(const tcsdn_model_t *m);
 /* columns of scores_out: linear n_rows (decision_function), gnb n_classes (joint log likelihood),
- * kmeans k (||c||^2 - 2 x.c), knn n_classes (neighbour votes / k, or distance-weighted votes normalised),
+ * kmeans k (||c||^2 - 2 x.c), knn n_classes (neighbour votes / k, or distance-weighted votes normalised, the weights
+ * 1 / distance in the handle's metric),
  * svc n_classes*(n_classes-1)/2
  * (libsvm's one-vs-one decision values), forest n_classes (predict_proba). */
 int tcsdn_model_score_cols(const tcsdn_model_t *m);
 int tcsdn_set_option(tcsdn_model_t *m, int32_t key, int64_t value);
-/* counters of the last predict on this handle: [0] kernels launched, [1] rows through the tensor-core
- * engine, [2] rows through the fp64 CUDA-core kernels, [3] exact fp64 re-evaluations of the knn filter (cumulative
- * since create), [4] knn engine: reference tiles multiplied per 512-row pass, times 1000 (cumulative average), [5] largest observed |tensor-core value - exact| / (the error model's denominator), times 2^40
+/* counters of the last predict on this handle: [0] kernels launched, [1] engine rows: rows through the tensor-core
+ * engine (manhattan and chebyshev handles: through the pruned CUDA-core kernel), [2] rows through the fp64 CUDA-core kernels, [3] exact fp64 re-evaluations of the knn filter (cumulative
+ * since create), [4] knn engine: reference tiles multiplied per 256-row pass (manhattan / chebyshev: tiles evaluated per 128-row pass of
+ * the pruned kernel), times 1000 (cumulative average), [5] largest observed |tensor-core value - exact| / (the error model's denominator), times 2^40
  * (cumulative, audit mode), [6] rows a certified fast path could not decide and handed to the fp64 definition
  * (GaussianNB fp32 pre-pass, svc engine, linear svc collapsed path; cumulative since create), [7] knn engine: rows whose label depended on a tie at
  * the k-th distance and were re-run by the index-order fp64 kernel (cumulative).  out has 8 slots.  Reading the
@@ -176,11 +196,11 @@ int tcsdn_predict(tcsdn_model_t *m, const void *x, int64_t n, int32_t d, int32_t
 
 /* KNeighborsClassifier.kneighbors(X, n_neighbors) (sk:neighbors/_base.py:750-960): per row of X the n_neighbors nearest
  * training rows, ind_out [n][n_neighbors] int64 training indices and dist_out (nullable) [n][n_neighbors] float64
- * euclidean distances, both where x_loc says.  The set is the one predict votes on: the rows sklearn's index-order heap
+ * distances in the handle's metric, both where x_loc says.  The set is the one predict votes on: the rows sklearn's index-order heap
  * keeps (ArgKmin, parallel_on_X; sk:utils/_heap.pyx), so with n_neighbors == k the vote of y[ind] is predict's label.
  * Each row is in ascending (distance, training index) order -- sklearn leaves equal distances in no defined order, this
- * call sorts them by index.  dist = sqrt(sum_f (x_f - t_f)^2), fp64, features in order, no FMA, correctly rounded sqrt;
- * float32 rows are widened first.  1 <= n_neighbors <= min(64, n_samples_fit); TCSDN_EINVAL otherwise, for a handle that
+ * call sorts them by index.  Euclidean: dist = sqrt(sum_f (x_f - t_f)^2), fp64, features in order, no FMA, correctly
+ * rounded sqrt; manhattan and chebyshev: dist = rdist (tcsdn_knn_create_metric); float32 rows are widened first.  1 <= n_neighbors <= min(64, n_samples_fit); TCSDN_EINVAL otherwise, for a handle that
  * is not a KNeighborsClassifier and under engine options 3 and 4.  Path, device, counters ([1] engine rows, [2] fp64
  * kernel rows, [7] index-order reruns) and non-finite rules are tcsdn_predict's: host pointers return TCSDN_ENONFINITE,
  * device pointers set the sticky flag tcsdn_sync_check reads.  Host pointers are processed through the same pipeline as tcsdn_predict. */

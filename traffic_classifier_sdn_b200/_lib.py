@@ -17,6 +17,8 @@ OPT_ENGINE, OPT_CHUNK_ROWS, OPT_CHECK_FINITE = 1, 2, 3
 OPT_SCORER_SHAPE, OPT_FOREST_SHAPE, OPT_FOREST_SORT, OPT_KNN_FLUSH_TILES, OPT_KNN_PRUNE = 4, 5, 6, 7, 8
 FLOW_STATE = 19
 KNN_UNIFORM, KNN_DISTANCE = 0, 1
+KNN_EUCLIDEAN, KNN_MANHATTAN, KNN_CHEBYSHEV = 0, 1, 2
+KNN_METRICS = {"euclidean": KNN_EUCLIDEAN, "manhattan": KNN_MANHATTAN, "chebyshev": KNN_CHEBYSHEV}
 SVC_LINEAR, SVC_POLY, SVC_RBF, SVC_SIGMOID = 0, 1, 2, 3
 SVC_KERNELS = {"linear": SVC_LINEAR, "poly": SVC_POLY, "rbf": SVC_RBF, "sigmoid": SVC_SIGMOID}
 COMM_ID_BYTES = 128
@@ -39,6 +41,8 @@ SIGNATURES = {
     "tcsdn_knn_create": (C.c_int, [_f64p, _i32p, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.POINTER(_vp)]),
     "tcsdn_knn_create_weighted": (C.c_int, [_f64p, _i32p, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                             C.POINTER(_vp)]),
+    "tcsdn_knn_create_metric": (C.c_int, [_f64p, _i32p, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                          C.POINTER(_vp)]),
     "tcsdn_svc_create": (C.c_int, [_f64p, _f64p, _f64p, _i32p, C.c_int32, C.c_int32, C.c_int32, C.c_double,
                                    C.POINTER(_vp)]),
     "tcsdn_svc_create_kernel": (C.c_int, [_f64p, _f64p, _f64p, _i32p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_double,

@@ -113,7 +113,8 @@ static void release_workspace(tcsdn_model *m, Workspace *w) {
     w->in_use = false;
 }
 
-// KNN predict and kneighbors: the engine when it can run the call, else the fp64 kernel (engine option 1 forces the latter).
+// KNN predict and kneighbors: the engine when it can run the call (euclidean: the tensor-core engine; manhattan / chebyshev:
+// the pruned CUDA-core kernel on its index), else the fp64 kernel (engine option 1 forces the latter).
 // `flag` (here and in run_device): where the kernels record non-finite rows -- the handle's sticky flag for device-pointer
 // calls (read by tcsdn_sync_check), the workspace's own for host-pointer calls (so that concurrent calls cannot see or clear
 // each other's)
@@ -121,8 +122,11 @@ static int run_knn(tcsdn_model *m, const void *x, int64_t n, int dtype, const Kn
     if (!m->opt_check_finite) flag = nullptr;
     if (m->opt_engine != 1 && knn_engine_usable(m, n, call)) return launch_knn_engine(m, x, n, dtype, call, flag, st);
     if (m->opt_engine >= 2) {
-        set_error(call.out == KnnOut::Neighbors ? "tensor-core engine forced but not usable for this model/batch/n_neighbors"
-                                                : "tensor-core engine forced but not usable for this model/batch");
+        if (m->knn_metric != Metric::L2)
+            set_error("pruned kernel forced but not usable for this model/batch/n_neighbors (n_features <= 12, k <= 32)");
+        else
+            set_error(call.out == KnnOut::Neighbors ? "tensor-core engine forced but not usable for this model/batch/n_neighbors"
+                                                    : "tensor-core engine forced but not usable for this model/batch");
         return TCSDN_EINVAL;
     }
     return launch_knn_exact(m, x, n, dtype, call, flag, st);
@@ -420,8 +424,17 @@ int tcsdn_knn_create(const double *fit_x, const int32_t *y, int64_t n_train, int
 
 int tcsdn_knn_create_weighted(const double *fit_x, const int32_t *y, int64_t n_train, int32_t d, int32_t n_classes, int32_t k,
                               int32_t weights, tcsdn_model_t **out) {
+    return tcsdn_knn_create_metric(fit_x, y, n_train, d, n_classes, k, weights, TCSDN_KNN_EUCLIDEAN, out);
+}
+
+int tcsdn_knn_create_metric(const double *fit_x, const int32_t *y, int64_t n_train, int32_t d, int32_t n_classes, int32_t k,
+                            int32_t weights, int32_t metric, tcsdn_model_t **out) {
     if (!out) { set_error("out handle pointer is NULL"); return TCSDN_EINVAL; }
     *out = nullptr;
+    if (metric != TCSDN_KNN_EUCLIDEAN && metric != TCSDN_KNN_MANHATTAN && metric != TCSDN_KNN_CHEBYSHEV) {
+        set_error("knn: metric must be TCSDN_KNN_EUCLIDEAN, TCSDN_KNN_MANHATTAN or TCSDN_KNN_CHEBYSHEV, got %d", metric);
+        return TCSDN_EINVAL;
+    }
     if (weights != TCSDN_KNN_UNIFORM && weights != TCSDN_KNN_DISTANCE) {
         set_error("knn: weights must be TCSDN_KNN_UNIFORM or TCSDN_KNN_DISTANCE, got %d", weights);
         return TCSDN_EINVAL;
@@ -434,7 +447,7 @@ int tcsdn_knn_create_weighted(const double *fit_x, const int32_t *y, int64_t n_t
         if (y[i] < 0 || y[i] >= n_classes) { set_error("knn: label index out of range"); return TCSDN_EINVAL; }
     tcsdn_model *m;
     TCSDN_TRY(model_base(&m, TCSDN_KIND_KNN, d, n_classes, n_classes));
-    m->n_train = n_train; m->k = k; m->knn_weights = weights;
+    m->n_train = n_train; m->k = k; m->knn_weights = weights; m->knn_metric = static_cast<Metric>(metric);
     int r = upload(&m->d_fit, fit_x, (size_t)n_train * d);
     if (r == TCSDN_OK) r = upload(&m->d_y, y, (size_t)n_train);
     if (r == TCSDN_OK) r = knn_engine_create(m);
@@ -542,6 +555,10 @@ int tcsdn_set_option(tcsdn_model_t *m, int32_t key, int64_t value) {
             if (value < 0 || value > 4) { set_error("engine option must be 0..4"); return TCSDN_EINVAL; }
             if (value >= 2 && m->kind == TCSDN_KIND_SVC && (m->svc_kernel == TCSDN_SVC_POLY || m->svc_kernel == TCSDN_SVC_SIGMOID)) {
                 set_error("engine options 2..4: poly and sigmoid SVC models have no fast path (the fp64 kernel runs every call)");
+                return TCSDN_EINVAL;
+            }
+            if (value >= 3 && m->kind == TCSDN_KIND_KNN && m->knn_metric != Metric::L2) {
+                set_error("engine options 3 and 4 audit the tensor-core engine, which manhattan and chebyshev models do not use");
                 return TCSDN_EINVAL;
             }
             m->opt_engine = value; return TCSDN_OK;

@@ -88,7 +88,30 @@ __device__ __forceinline__ void peer_flag_wait(const GatherOut &G, int which, un
     }
 }
 
-// One query's m kept neighbours (squared distance, training index), slot i at values[i * ST], sorted in place into the
+// KNeighborsClassifier's metric, fixed when the handle is created (tcsdn_knn_create_metric).  rdist is what the kernels rank
+// by, in sklearn's arithmetic (sk:metrics/_dist_metrics.pyx.tp, features in order from 0.0, fp64, no FMA):
+//   L2    sum_j (x_j - t_j)^2          (EuclideanDistance.rdist; the distance is its correctly rounded sqrt)
+//   L1    sum_j |x_j - t_j|            (ManhattanDistance.dist)
+//   Linf  max_j |x_j - t_j|            (ChebyshevDistance.dist)
+enum class Metric { L2 = TCSDN_KNN_EUCLIDEAN, L1 = TCSDN_KNN_MANHATTAN, Linf = TCSDN_KNN_CHEBYSHEV };
+
+// the running rdist after one more feature pair (x, t)
+template <Metric M>
+__device__ __forceinline__ double rdist(double acc, double x, double t) {
+    const double df = __dsub_rn(x, t);
+    if constexpr (M == Metric::L2) return __dadd_rn(acc, __dmul_rn(df, df));
+    else if constexpr (M == Metric::L1) return __dadd_rn(acc, fabs(df));
+    else return fmax(acc, fabs(df));
+}
+
+// rdist -> the distance kneighbors reports and distance weights divide by
+template <Metric M>
+__device__ __forceinline__ double to_dist(double r) {
+    if constexpr (M == Metric::L2) return __dsqrt_rn(r);
+    else return r;
+}
+
+// One query's m kept neighbours (rdist, training index), slot i at values[i * ST], sorted in place into the
 // canonical ascending (distance, index) order.  m <= 64: an insertion sort is all it needs.
 template <int ST>
 __device__ __forceinline__ void knn_sort_neighbors(double *values, int32_t *indices, int m) {
@@ -105,14 +128,14 @@ __device__ __forceinline__ void knn_sort_neighbors(double *values, int32_t *indi
     }
 }
 
-// KNeighbors.kneighbors: the neighbours in canonical order, written as one row of ind (and of dist = sqrt, correctly rounded,
-// when dist is non-null)
-template <int ST>
+// KNeighbors.kneighbors: the neighbours in canonical order, written as one row of ind (and of dist = to_dist<M>, when dist is
+// non-null)
+template <Metric M, int ST>
 __device__ __forceinline__ void knn_write_neighbors(double *values, int32_t *indices, int m, int64_t *ind, double *dist) {
     knn_sort_neighbors<ST>(values, indices, m);
     for (int i = 0; i < m; ++i) {
         ind[i] = indices[i * ST];
-        if (dist) dist[i] = __dsqrt_rn(values[i * ST]);
+        if (dist) dist[i] = to_dist<M>(values[i * ST]);
     }
 }
 
@@ -163,23 +186,23 @@ __device__ __forceinline__ double np_sum(const F &term, int n) {
 }
 
 // KNeighborsClassifier(weights='distance') for one query (sk:neighbors/_base.py:74-114, _classification.py:281-307,398-410,
-// sk:utils/extmath.py:791-862): values / indices hold the k kept neighbours as (squared distance, training index), slot i at
+// sk:utils/extmath.py:791-862): values / indices hold the k kept neighbours as (rdist, training index), slot i at
 // [i * ST]; y maps a training index to its class.  The slots are sorted into canonical (distance, index) order and then
 // overwritten with (weight, class):
-//   weight  w_i = 1 / sqrt(d_i), both correctly rounded; if any d_i == 0, w_i = 1 where d_i == 0 and 0 elsewhere
+//   weight  w_i = 1 / to_dist<M>(d_i), both correctly rounded; if any d_i == 0, w_i = 1 where d_i == 0 and 0 elsewhere
 //   label   per class c, W_c = numpy's row sum (np_sum_block) of the k columns of template_c = (w_i if y_i == c else 0.0);
 //           the lowest class with the largest W_c (weighted_mode: strict > in class order)
 //   proba   (non-null: C entries) P_c = 0.0 + the w_i of class c, sequentially in column order; P_c / (numpy's row sum of
 //           P_0 .. P_{C-1}).  The two sums associate differently, so the label may differ from argmax(proba) in the last
 //           bit exactly as sklearn's may.
-template <int ST>
+template <Metric M, int ST>
 __device__ __forceinline__ void knn_weighted_vote(double *values, int32_t *indices, int k, int C, const int32_t *__restrict__ y,
                                                   int32_t *label, double *proba) {
     knn_sort_neighbors<ST>(values, indices, k);
     const bool zero = values[0] == 0.0;   // sorted: a zero distance comes first
     for (int i = 0; i < k; ++i) {
         const double v = values[i * ST];
-        values[i * ST] = zero ? (v == 0.0 ? 1.0 : 0.0) : __ddiv_rn(1.0, __dsqrt_rn(v));
+        values[i * ST] = zero ? (v == 0.0 ? 1.0 : 0.0) : __ddiv_rn(1.0, to_dist<M>(v));
         indices[i * ST] = y[indices[i * ST]];
     }
     if (proba)
@@ -211,19 +234,19 @@ __device__ __forceinline__ void knn_weighted_vote(double *values, int32_t *indic
 // weights='distance' handles) or the neighbours themselves (kneighbors)
 enum class KnnOut { Vote, WeightedVote, Neighbors };
 
-// Query q's result from its k kept neighbours (values / indices: squared distance and index, slot i at [i * ST]).  y maps an
+// Query q's result from its k kept neighbours (values / indices: rdist in metric M and index, slot i at [i * ST]).  y maps an
 // index to its class, so it must match what the indices count: training labels for training indices, the engine's labels in
 // tile order for its tile positions (Vote only: the other two order equal distances by training index).
 //   Vote          labels[q] = the lowest class with the most neighbours; proba (nullable) [n][C] the class fractions
 //   WeightedVote  labels[q] and proba[q] (nullable) from knn_weighted_vote
 //   Neighbors     nb_ind [n][k] the indices and nb_dist [n][k] (nullable) the distances, by knn_write_neighbors
-template <KnnOut OUT, int ST>
+template <Metric M, KnnOut OUT, int ST>
 __device__ __forceinline__ void knn_finish(double *values, int32_t *indices, int k, int C, const int32_t *__restrict__ y, int64_t q,
                                            int32_t *labels, double *proba, int64_t *nb_ind, double *nb_dist) {
     if constexpr (OUT == KnnOut::Neighbors) {
-        knn_write_neighbors<ST>(values, indices, k, nb_ind + q * k, nb_dist ? nb_dist + q * k : nullptr);
+        knn_write_neighbors<M, ST>(values, indices, k, nb_ind + q * k, nb_dist ? nb_dist + q * k : nullptr);
     } else if constexpr (OUT == KnnOut::WeightedVote) {
-        knn_weighted_vote<ST>(values, indices, k, C, y, labels + q, proba ? proba + q * C : nullptr);
+        knn_weighted_vote<M, ST>(values, indices, k, C, y, labels + q, proba ? proba + q * C : nullptr);
     } else {
         int best = 0, arg = 0;
         for (int c = 0; c < C; ++c) {
@@ -284,6 +307,7 @@ struct tcsdn_model {
     int64_t n_train = 0;
     int k = 0;
     int knn_weights = 0;       // TCSDN_KNN_UNIFORM or TCSDN_KNN_DISTANCE (predict only; kneighbors ignores it)
+    tcsdn::Metric knn_metric = tcsdn::Metric::L2;
 
     // ---- svc
     double *d_sv = nullptr;      // [n_sv][d]

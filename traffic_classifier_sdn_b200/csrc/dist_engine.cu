@@ -31,6 +31,18 @@
 // kneighbors (KnnOut::Neighbors) returns the SET, so there any row left out at the final k-th distance sends the query to that
 // kernel.  The distance-weighted vote (KnnOut::WeightedVote) keeps the class rule: equally distant rows weigh the same, so
 // where every tied row carries one class, every choice gives the same (weight, class) columns in canonical order.
+// Manhattan and chebyshev (knn_metric_kernel).  The same spatial index, built in the handle's metric at create time (tile
+// centres, radii r_t >= max rdist(row, c_t), the per-home-tile order and the chunk bounds; no bf16 tile images), searched by
+// fp64 CUDA cores: rdist needs no MMA middle term, so every computed distance is the definition's bits and there is no
+// filter to re-evaluate.  Both metrics satisfy the triangle inequality, so for a query x of a pass with first row x0 and any
+// row t of tile t:  rdist(x, t) >= rdist(x0, c_t) - r_t - rdist(x, x0).  A tile is skipped for x only when that bound
+// exceeds x's current k-th rdist (strictly: a row at exactly the k-th value is still seen, and only such rows are ever
+// tie-noted).  Roundings: a computed rdist of d <= 12 terms is within a relative (d + 1) 2^-53 < 2^-40 of the exact one
+// (each |x - t| is one rounded subtraction, manhattan adds up to 12 such terms, chebyshev's max is exact), so the kernel takes
+// rdist(x0, c_t) (1 - 2^-40) rounded down, rdist(x, x0) (1 + 2^-40) rounded up, r_t from the host with a factor 1 + 1e-9,
+// subtracts rounding down, and skips only if that bound times (1 - 2^-40), rounded down, is still above the k-th value --
+// then every computed rdist of the tile is too.  A non-finite x0 or row prunes nothing.  Ties at the final k-th rdist follow
+// the tensor-core engine's rule below, with the same tie list and the same index-order kernel.
 // SVC uses acc directly, for LABELS only: e = -gamma log2(e) (acc + ||x' - c'_j||^2), K = ex2(e), C-1 fp32 FMAs per pair into
 // the running sums of the support vector's class, tile sums promoted to fp64.  To keep the fp32 accumulation error small
 // where K is not negligible, support vectors are re-ordered inside their class into spatially compact tiles and every tile
@@ -148,6 +160,7 @@ struct EngineState {
 };
 
 struct KnnEngine : EngineState {
+    Metric metric = Metric::L2;         // the handle's: L2 runs knn_engine_kernel, L1 / Linf knn_metric_kernel (no tile images)
     int32_t *d_tile_rows = nullptr;     // per tile: number of real rows
     double *d_refpad = nullptr;         // training rows in tile order, row stride padded to kEMaxD doubles (16 B loads)
     // pruning (see "KNN: spatial order and pruning" in the file header)
@@ -156,6 +169,7 @@ struct KnnEngine : EngineState {
     double *d_kd_split = nullptr;       // split value (rows with x[dim] < split go left)
     int32_t *d_leaf_tile = nullptr;     // leaf -> the tile its rows sit in
     int n_leaves = 0;
+    // the three tables below are in the handle's metric (L2: the euclidean distance, L1 / Linf: rdist)
     double *d_tcent = nullptr;          // [n_tiles][d] tile centres
     double *d_trad = nullptr;           // [n_tiles] tile radii (max distance of a row from the centre, rounded up)
     uint16_t *d_nbr = nullptr;          // [n_tiles][n_tiles]: per home tile, all tiles by centre distance (nullptr: pruning off)
@@ -955,11 +969,11 @@ knn_engine_kernel(const __grid_constant__ KnnArgs A, const T *__restrict__ X, in
                         if constexpr (!kKnb) labels[row] = -1;
                         A.tie_list[atomicAdd(A.tie_count, 1)] = (int32_t)row;
                     } else if constexpr (OUT == KnnOut::Vote) {
-                        knn_finish<OUT, ST>(hv, hi, A.k, A.C, A.ypos, row, labels, scores, nullptr, nullptr);
+                        knn_finish<Metric::L2, OUT, ST>(hv, hi, A.k, A.C, A.ypos, row, labels, scores, nullptr, nullptr);
                     } else {
                         // equal distances are ordered by TRAINING index: map the tile positions before the sort
                         for (int i = 0; i < A.k; ++i) hi[i * ST] = A.pos_orig[hi[i * ST]];
-                        knn_finish<OUT, ST>(hv, hi, A.k, A.C, A.y, row, labels, scores, A.nb_ind, A.nb_dist);
+                        knn_finish<Metric::L2, OUT, ST>(hv, hi, A.k, A.C, A.y, row, labels, scores, A.nb_ind, A.nb_dist);
                     }
                 }
                 {   // one counter update per warp
@@ -970,6 +984,198 @@ knn_engine_kernel(const __grid_constant__ KnnArgs A, const T *__restrict__ X, in
         }
         if (A.flag && nf != nf) atomicOr(A.flag, 1);
     }
+}
+
+// ------------------------------------------------------------------------------------------------ KNN: manhattan, chebyshev
+// knn_metric_kernel (the file header's "Manhattan and chebyshev"): fp64 CUDA cores on the engine's spatial index.  A CTA takes
+// a pass of kMThreads sorted queries, one per thread, and walks the tiles in the home tile's order: per chunk of kMThreads
+// tiles every thread tests one tile against the pass-wide bound, the survivors are compacted, then each is tested again
+// with the current k-th rdist of every warp, staged in shared memory (64 x 12 fp64, read by broadcast) and evaluated by the
+// lanes whose own test does not rule it out.
+constexpr int kMThreads = 128;
+// smaller batches run on the fp64 kernel (knn.cu).  Bench model (50k x 12, k = 5), H100 80GB HBM3 at 700 W,
+// tools/knn_metric_time.py: at 1 024 rows the pruned kernel takes 7.6 ms against 13.4 ms (manhattan) and 14.7 against 17.2 ms
+// (chebyshev); smaller batches were not measured
+constexpr int64_t kMetricMinRows = 1024;
+constexpr double kMShrink = 1.0 - 1.0 / 1099511627776.0;   // 1 -+ 2^-40: the relative error of an fp64 rdist of <= 12 terms
+constexpr double kMGrow = 1.0 + 1.0 / 1099511627776.0;     // (< 13 x 2^-53) with room to spare, taken in the safe direction
+
+template <Metric M>
+__device__ __forceinline__ double rdist_d(const double (&x)[kEMaxD], const double *__restrict__ t, int d) {
+    double acc = 0.0;
+#pragma unroll
+    for (int j = 0; j < kEMaxD; ++j)
+        if (j < d) acc = rdist<M>(acc, x[j], t[j]);
+    return acc;
+}
+
+// no row of a tile whose rows are at least `gap` from x0 (a lower bound, rounded down) can change the heap of a query within
+// `rho` of x0 (an upper bound, rounded up) whose k-th rdist is kth: every computed rdist of such a pair exceeds kth
+__device__ __forceinline__ bool metric_far(double gap, double rho, double kth) {
+    return __dmul_rd(__dsub_rd(gap, rho), kMShrink) > kth;
+}
+
+template <typename T, Metric M, KnnOut OUT>
+__global__ void __launch_bounds__(kMThreads, 4) knn_metric_kernel(const __grid_constant__ KnnArgs A, const T *__restrict__ X,
+                                                                 int32_t *__restrict__ labels, double *__restrict__ scores,
+                                                                 unsigned long long *__restrict__ counters) {
+    static_assert(M != Metric::L2, "euclidean handles run knn_engine_kernel");
+    constexpr bool kKnb = OUT == KnnOut::Neighbors;   // the output is the neighbour SET
+    constexpr int kW = kMThreads / 32;
+    __shared__ __align__(16) double s_tile[kEN * kEMaxD];   // the tile being evaluated (refpad layout)
+    __shared__ double s_gap[kMThreads];                     // the chunk's surviving tiles, in walk order, and their gaps
+    __shared__ int s_t[kMThreads];
+    __shared__ double s_kth[kW];                            // per warp: largest current k-th rdist of its live rows
+    __shared__ double s_rho[kW];
+    __shared__ int s_cnt[kW];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const bool prune = A.qperm != nullptr;
+    const int n_chunks = (A.n_tiles + kMThreads - 1) / kMThreads, n_lb = (A.n_tiles + 31) >> 5;
+    const int64_t n_pass = (A.n + kMThreads - 1) / kMThreads;
+    auto warp_max = [](double v) {
+#pragma unroll
+        for (int o = 16; o; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
+        return v;
+    };
+    auto cta_max = [](const double *w) {
+        double v = w[0];
+#pragma unroll
+        for (int i = 1; i < kW; ++i) v = fmax(v, w[i]);
+        return v;
+    };
+    float nf = 0.f;
+    unsigned long long n_eval = 0, n_passes = 0;
+    for (int64_t ps = blockIdx.x; ps < n_pass; ps += gridDim.x, ++n_passes) {
+        const int64_t slot = ps * kMThreads + tid;
+        const bool live = slot < A.n;
+        const int64_t row = !live ? 0 : (prune ? (int64_t)A.qperm[slot] : slot);   // the query this thread owns
+        const int64_t src0 = prune ? (int64_t)A.qperm[ps * kMThreads] : ps * kMThreads;
+        double x[kEMaxD], x0[kEMaxD];   // zero beyond d: the refpad columns there are zero too, and |0 - 0| changes no rdist
+        bool fin0 = true;
+#pragma unroll
+        for (int j = 0; j < kEMaxD; ++j) {
+            x[j] = 0.0;
+            x0[j] = 0.0;
+            if (j < A.d) {
+                if (live) {
+                    const T v = X[row * A.d + j];
+                    nf += static_cast<float>(v * static_cast<T>(0));
+                    x[j] = static_cast<double>(v);
+                }
+                x0[j] = static_cast<double>(X[src0 * A.d + j]);
+                fin0 &= isfinite(x0[j]);
+            }
+        }
+        // rho >= this row's distance from x0; a non-finite row or x0 prunes nothing
+        double rho = __dmul_ru(rdist_d<M>(x, x0, A.d), kMGrow);
+        if (!(rho <= DBL_MAX) || !fin0) rho = INFINITY;
+        if (!live) rho = 0.0;
+        double hv[kEMaxK];
+        int32_t hi[kEMaxK];
+        for (int i = 0; i < A.k; ++i) { hv[i] = DBL_MAX; hi[i] = 0; }
+        double hv0 = DBL_MAX, tie_val = -1.0;
+        int tie_cls = -1;
+        // rows left out of the heap at the root's value: the tie rule of knn_engine_kernel
+        auto tie_note = [&](double v, int32_t pos) {
+            const int c = A.ypos[pos];
+            if (v != tie_val) { tie_val = v; tie_cls = c; }
+            else if (tie_cls != c) tie_cls = -2;
+        };
+        auto offer = [&](double dv, int32_t pos) {
+            if (dv < hv0) {
+                const double ev = hv0;
+                const int32_t ei = hi[0];
+                knn_heap_push<1>(hv, hi, A.k, dv, pos);
+                hv0 = hv[0];
+                if (hv0 == ev) tie_note(ev, ei);
+            } else if (dv == hv0) tie_note(dv, pos);
+        };
+        const double wrho = warp_max(rho);
+        __syncthreads();                                   // the previous pass is done with the shared arrays
+        if (lane == 0) { s_rho[warp] = wrho; s_kth[warp] = DBL_MAX; }
+        __syncthreads();
+        const double rho_max = cta_max(s_rho);
+        const int home = prune ? A.leaf_tile[A.qkey[src0]] : 0;
+        // >= the distance of every row of the pass from the home tile's centre (the chunk bound's reference point)
+        const double base = prune ? __dadd_ru(__dmul_ru(rdist_d<M>(x0, A.tcent + (size_t)home * A.d, A.d), kMGrow), rho_max) : 0.0;
+        for (int c = 0; c < n_chunks; ++c) {
+            const double kmax = cta_max(s_kth);
+            // chunk_lb: every tile from this chunk on is at least that far from c_home, minus its radius
+            if (prune && A.nbr && metric_far((double)A.chunk_lb[(size_t)home * n_lb + c * (kMThreads / 32)], base, kmax)) break;
+            const int p = c * kMThreads + tid;
+            int t = -1;
+            double gap = -INFINITY;
+            if (p < A.n_tiles) {
+                t = p;
+                if (prune) {
+                    if (A.nbr) {
+                        t = A.nbr[(size_t)home * A.n_tiles + p];
+                    } else {   // no tile-by-tile table: outwards from the home tile in kd order, as knn_engine_kernel's producer
+                        const int lo = home, hi2 = A.n_tiles - 1 - home, mside = min(lo, hi2);
+                        if (p <= 2 * mside) { const int kk = (p + 1) >> 1; t = (p & 1) ? home + kk : home - kk; }
+                        else { const int jj = p - 2 * mside; t = hi2 > lo ? home + mside + jj : home - mside - jj; }
+                    }
+                    // <= rdist(x0, row) for every row of tile t
+                    gap = __dsub_rd(__dmul_rd(rdist_d<M>(x0, A.tcent + (size_t)t * A.d, A.d), kMShrink), A.trad[t]);
+                    if (metric_far(gap, rho_max, kmax)) t = -1;
+                }
+            }
+            const unsigned keep = __ballot_sync(0xffffffffu, t >= 0);
+            if (lane == 0) s_cnt[warp] = __popc(keep);
+            __syncthreads();
+            int off = 0, total = 0;
+#pragma unroll
+            for (int w = 0; w < kW; ++w) { off += w < warp ? s_cnt[w] : 0; total += s_cnt[w]; }
+            if (t >= 0) {
+                const int i = off + __popc(keep & ((1u << lane) - 1u));
+                s_t[i] = t;
+                s_gap[i] = gap;
+            }
+            __syncthreads();
+            for (int i = 0; i < total; ++i) {
+                const int ti = s_t[i];
+                const double gi = s_gap[i];
+                if (prune && metric_far(gi, rho_max, cta_max(s_kth))) continue;   // the same for every thread
+                const double2 *src = reinterpret_cast<const double2 *>(A.refpad + (size_t)ti * kEN * kEMaxD);
+                for (int e = tid; e < kEN * kEMaxD / 2; e += kMThreads) reinterpret_cast<double2 *>(s_tile)[e] = src[e];
+                __syncthreads();
+                if (live && !(prune && metric_far(gi, rho, hv0))) {
+                    const int rows = A.tile_rows[ti];
+                    for (int r = 0; r < rows; ++r) {
+                        double dv = 0.0;
+#pragma unroll
+                        for (int j = 0; j < kEMaxD; ++j) dv = rdist<M>(dv, x[j], s_tile[r * kEMaxD + j]);
+                        offer(dv, ti * kEN + r);
+                    }
+                }
+                ++n_eval;
+                const double wk = warp_max(live ? hv0 : 0.0);
+                if (lane == 0) s_kth[warp] = wk;
+                __syncthreads();
+            }
+        }
+        if (live) {
+            // as knn_engine_kernel: a row left out at exactly the final k-th rdist sends the query to the index-order kernel when
+            // the choice among the tied rows can matter (the vote: their classes differ; kneighbors: always)
+            bool tied = false;
+            if (tie_val == hv0) {
+                tied = kKnb || tie_cls < 0;
+                if constexpr (!kKnb)
+                    for (int i = 0; i < A.k; ++i) tied |= (hv[i] == hv0 && A.ypos[hi[i]] != tie_cls);
+            }
+            if (tied) {
+                if constexpr (!kKnb) labels[row] = -1;
+                A.tie_list[atomicAdd(A.tie_count, 1)] = (int32_t)row;
+            } else if constexpr (OUT == KnnOut::Vote) {
+                knn_finish<M, OUT, 1>(hv, hi, A.k, A.C, A.ypos, row, labels, scores, nullptr, nullptr);
+            } else {
+                for (int i = 0; i < A.k; ++i) hi[i] = A.pos_orig[hi[i]];   // equal distances go by TRAINING index
+                knn_finish<M, OUT, 1>(hv, hi, A.k, A.C, A.y, row, labels, scores, A.nb_ind, A.nb_dist);
+            }
+        }
+    }
+    if (tid == 0 && counters) { atomicAdd(counters + 2, n_eval); atomicAdd(counters + 3, n_passes); }
+    if (A.flag && nf != nf) atomicOr(A.flag, 1);
 }
 
 // SVC(rbf): the producer's lane 0 streams every tile in order; 4 epilogue warps (one warpgroup, both query tiles), two query
@@ -1449,16 +1655,32 @@ KnnEngine::~KnnEngine() {
 
 SvcEngine::~SvcEngine() { cudaFree(d_tile_class); }
 
+// distance between two points in the metric of a KNN handle, on the host: L2 the euclidean distance, L1 / Linf rdist
+static double host_dist(Metric metric, const double *a, const double *b, int d) {
+    double acc = 0.0;
+    for (int j = 0; j < d; ++j) {
+        const double df = a[j] - b[j];
+        if (metric == Metric::L2) acc += df * df;
+        else if (metric == Metric::L1) acc += std::fabs(df);
+        else acc = std::max(acc, std::fabs(df));
+    }
+    return metric == Metric::L2 ? std::sqrt(acc) : acc;
+}
+
+// The spatial index of a KNN handle, in its metric: kd order and tiles of 64 rows, the fp64 rows and labels in tile order,
+// the kd tree of the query sort, tile centres and radii, and per home tile the tiles by centre distance with the chunk
+// bounds.  Euclidean handles also get the bf16 tile images of the tensor-core engine and their norms (tile_tn).
 int knn_engine_create(tcsdn_model *m) {
     m->engine = nullptr;
     const int d = m->d;
     if (d > kEMaxD || m->k > kEMaxK) return TCSDN_OK;     // engine not applicable: fp64 kernels only
     const int64_t nref = m->n_train;
+    const Metric metric = m->knn_metric;
     std::vector<double> ref, center;
     TCSDN_TRY(host_rows(m->d_fit, nref, d, ref, center));
     KnnEngine *E = new KnnEngine();
     m->engine = E;   // from here on, what an error return leaves behind is freed by engine_destroy (tcsdn_destroy)
-    E->tile_bytes = kETileB;
+    E->metric = metric;
     // tile plan: kd order (spatially compact tiles: whole tiles can be skipped, see the file header)
     std::vector<int32_t> row0, rows, order((size_t)nref);
     for (int64_t i = 0; i < nref; ++i) order[(size_t)i] = (int32_t)i;
@@ -1467,14 +1689,21 @@ int knn_engine_create(tcsdn_model *m) {
     kd_build(ref, d, order, 0, (size_t)nref, kd);
     for (int64_t r = 0; r < nref; r += kEN) { row0.push_back((int32_t)r); rows.push_back((int32_t)std::min<int64_t>(kEN, nref - r)); }
     const int nt = E->n_tiles = (int)row0.size();
-    std::vector<unsigned char> img((size_t)nt * E->tile_bytes, 0);
-    std::vector<float> tile_tn((size_t)nt);
-    for (int t = 0; t < nt; ++t) {
-        const double rmax2 = pack_tile(img.data() + (size_t)t * E->tile_bytes, ref, &order[(size_t)row0[t]], rows[t], d,
-                                       center.data(), nullptr, 1.0 - (double)kKappa, true);
-        tile_tn[(size_t)t] = std::nextafterf(static_cast<float>(rmax2), INFINITY);
+    if (metric == Metric::L2) {
+        E->tile_bytes = kETileB;
+        std::vector<unsigned char> img((size_t)nt * E->tile_bytes, 0);
+        std::vector<float> tile_tn((size_t)nt);
+        for (int t = 0; t < nt; ++t) {
+            const double rmax2 = pack_tile(img.data() + (size_t)t * E->tile_bytes, ref, &order[(size_t)row0[t]], rows[t], d,
+                                           center.data(), nullptr, 1.0 - (double)kKappa, true);
+            tile_tn[(size_t)t] = std::nextafterf(static_cast<float>(rmax2), INFINITY);
+        }
+        TCSDN_TRY(upload_common(E, img, center));
+        TCSDN_TRY(upload(&E->d_tile_tn, tile_tn.data(), tile_tn.size()));
+    } else {
+        const unsigned long long zero4[4] = {};
+        TCSDN_TRY(upload(&E->d_counters, zero4, 4));
     }
-    TCSDN_TRY(upload_common(E, img, center));
     TCSDN_TRY(upload(&E->d_tile_rows, rows.data(), rows.size()));
     // exact re-evaluation reads the original rows with 16-byte loads: even row stride; rows in TILE order (a candidate is
     // (tile, column)), labels likewise
@@ -1491,8 +1720,8 @@ int knn_engine_create(tcsdn_model *m) {
     TCSDN_TRY(upload(&E->d_refpad, pad.data(), pad.size()));
     TCSDN_TRY(upload(&E->d_ypos, ypos.data(), ypos.size()));
     TCSDN_TRY(upload(&E->d_pos_orig, pos_orig.data(), pos_orig.size()));
-    TCSDN_TRY(upload(&E->d_tile_tn, tile_tn.data(), tile_tn.size()));
-    // pruning tables: tile centres and radii, the kd tree, and per home tile the tiles by centre distance
+    // pruning tables: tile centres and radii, the kd tree, and per home tile the tiles by centre distance.  The host sums
+    // round to nearest; the factors 1 +- 1e-9 cover their error (<= 12 terms: below 2^-48 relative) in the safe direction.
     std::vector<double> tcent((size_t)nt * d, 0.0), trad((size_t)nt, 0.0);
     for (int t = 0; t < nt; ++t) {
         for (int j = 0; j < d; ++j) {
@@ -1500,13 +1729,10 @@ int knn_engine_create(tcsdn_model *m) {
             for (int r = 0; r < rows[t]; ++r) a += ref[(size_t)order[(size_t)(row0[t] + r)] * d + j];
             tcent[(size_t)t * d + j] = a / rows[t];
         }
-        double r2 = 0.0;
-        for (int r = 0; r < rows[t]; ++r) {
-            double a = 0.0;
-            for (int j = 0; j < d; ++j) { const double df = ref[(size_t)order[(size_t)(row0[t] + r)] * d + j] - tcent[(size_t)t * d + j]; a += df * df; }
-            r2 = std::max(r2, a);
-        }
-        trad[(size_t)t] = std::sqrt(r2) * (1.0 + 1e-9) + 1e-300;
+        double rmax = 0.0;
+        for (int r = 0; r < rows[t]; ++r)
+            rmax = std::max(rmax, host_dist(metric, &ref[(size_t)order[(size_t)(row0[t] + r)] * d], &tcent[(size_t)t * d], d));
+        trad[(size_t)t] = rmax * (1.0 + 1e-9) + 1e-300;
     }
     TCSDN_TRY(upload(&E->d_tcent, tcent.data(), tcent.size()));
     TCSDN_TRY(upload(&E->d_trad, trad.data(), trad.size()));
@@ -1521,11 +1747,7 @@ int knn_engine_create(tcsdn_model *m) {
         std::vector<float> clb((size_t)nt * nch);
         std::vector<std::pair<double, int>> byd((size_t)nt);
         for (int h = 0; h < nt; ++h) {
-            for (int t = 0; t < nt; ++t) {
-                double a = 0.0;
-                for (int j = 0; j < d; ++j) { const double df = tcent[(size_t)h * d + j] - tcent[(size_t)t * d + j]; a += df * df; }
-                byd[(size_t)t] = {std::sqrt(a), t};
-            }
+            for (int t = 0; t < nt; ++t) byd[(size_t)t] = {host_dist(metric, &tcent[(size_t)h * d], &tcent[(size_t)t * d], d), t};
             std::sort(byd.begin(), byd.end());
             double suffix = 1e300;   // min over positions >= i of (centre distance - radius), rounded down
             for (int i = nt - 1; i >= 0; --i) {
@@ -1671,6 +1893,7 @@ bool engine_usable(const tcsdn_model *m, int64_t n, bool want_scores) {
         if (want_scores != (m->opt_engine >= 3)) return false; // decision values: fp64 kernel; audit modes fill scores
     } else if (m->opt_engine == 4) return false;
     if (m->opt_engine >= 2) return true;
+    if (m->kind == TCSDN_KIND_KNN && static_cast<const KnnEngine *>(m->engine)->metric != Metric::L2) return n >= kMetricMinRows;
     return n >= 4096;   // below this the fp64 CUDA-core kernels (latency path) are faster than filling every SM with 256-row passes
 }
 
@@ -1690,6 +1913,17 @@ static unsigned engine_grid(const tcsdn_model *m, int64_t n) {   // persistent: 
 template <typename T, bool AUDIT, KnnOut OUT>
 static auto knn_kernel(bool heap_smem) {
     return heap_smem ? knn_engine_kernel<T, true, AUDIT, OUT> : knn_engine_kernel<T, false, AUDIT, OUT>;
+}
+
+template <typename T, Metric M>
+static auto metric_kernel(KnnOut out) {
+    return out == KnnOut::Neighbors      ? knn_metric_kernel<T, M, KnnOut::Neighbors>
+           : out == KnnOut::WeightedVote ? knn_metric_kernel<T, M, KnnOut::WeightedVote>
+                                         : knn_metric_kernel<T, M, KnnOut::Vote>;
+}
+template <typename T>
+static auto metric_kernel(Metric metric, KnnOut out) {
+    return metric == Metric::L1 ? metric_kernel<T, Metric::L1>(out) : metric_kernel<T, Metric::Linf>(out);
 }
 
 template <typename T>
@@ -1741,21 +1975,26 @@ static int knn_engine_run(tcsdn_model *m, const T *x, int64_t n, const KnnCall &
         A.nbr = E->d_nbr;   // nullptr beyond kEMaxPruneTiles: the producer walks outwards in kd order instead
         A.qperm = perm; A.qkey = key; A.leaf_tile = E->d_leaf_tile;
     }
-    const size_t smem = e_smem_bytes(E->tile_bytes) + kERows * (size_t)kEListCap * sizeof(uint16_t) +
-                        (heap_smem ? kERows * (size_t)call.k * 12 : 0);
-    decltype(&knn_engine_kernel<T, false, false, KnnOut::Vote>) kern;
-    if (A.maxratio) {
-        if (call.out != KnnOut::Vote) { set_error("knn engine: kneighbors and distance weights have no audit mode"); return TCSDN_EINVAL; }
-        kern = knn_kernel<T, true, KnnOut::Vote>(heap_smem);
-    } else if (call.out == KnnOut::Vote) {
-        kern = knn_kernel<T, false, KnnOut::Vote>(heap_smem);
-    } else if (call.out == KnnOut::WeightedVote) {
-        kern = knn_kernel<T, false, KnnOut::WeightedVote>(heap_smem);
+    if (E->metric != Metric::L2) {   // manhattan / chebyshev: the CUDA-core kernel on the same index
+        const int64_t grid = std::min<int64_t>((n + kMThreads - 1) / kMThreads, (int64_t)m->sm_count * 8);
+        metric_kernel<T>(E->metric, call.out)<<<(unsigned)grid, kMThreads, 0, st>>>(A, x, call.labels, call.scores, E->d_counters);
     } else {
-        kern = knn_kernel<T, false, KnnOut::Neighbors>(heap_smem);
+        const size_t smem = e_smem_bytes(E->tile_bytes) + kERows * (size_t)kEListCap * sizeof(uint16_t) +
+                            (heap_smem ? kERows * (size_t)call.k * 12 : 0);
+        decltype(&knn_engine_kernel<T, false, false, KnnOut::Vote>) kern;
+        if (A.maxratio) {
+            if (call.out != KnnOut::Vote) { set_error("knn engine: kneighbors and distance weights have no audit mode"); return TCSDN_EINVAL; }
+            kern = knn_kernel<T, true, KnnOut::Vote>(heap_smem);
+        } else if (call.out == KnnOut::Vote) {
+            kern = knn_kernel<T, false, KnnOut::Vote>(heap_smem);
+        } else if (call.out == KnnOut::WeightedVote) {
+            kern = knn_kernel<T, false, KnnOut::WeightedVote>(heap_smem);
+        } else {
+            kern = knn_kernel<T, false, KnnOut::Neighbors>(heap_smem);
+        }
+        TCSDN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        kern<<<engine_grid(m, n), kEKnnThreads, smem, st>>>(A, x, call.labels, call.scores, E->d_counters);
     }
-    TCSDN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kern<<<engine_grid(m, n), kEKnnThreads, smem, st>>>(A, x, call.labels, call.scores, E->d_counters);
     TCSDN_CUDA(cudaGetLastError());
     m->stats[0] += 1;
     m->stats[1] += n;
@@ -1837,7 +2076,8 @@ void engine_read_stats(const tcsdn_model *m, int64_t *out) {
             out[4] = c4[3] ? (int64_t)(1000.0 * (double)c4[2] / (double)c4[3]) : 0;
         }
     }
-    if (cudaMemcpy(&v, E->d_maxratio, sizeof(v), cudaMemcpyDeviceToHost) == cudaSuccess) out[5] = (int64_t)((double)v * 1099511627776.0);
+    if (E->d_maxratio && cudaMemcpy(&v, E->d_maxratio, sizeof(v), cudaMemcpyDeviceToHost) == cudaSuccess)   // none: L1 / Linf
+        out[5] = (int64_t)((double)v * 1099511627776.0);
 }
 
 }  // namespace tcsdn

@@ -3,7 +3,8 @@
 //   sk:metrics/_pairwise_distances_reduction/_argkmin.pyx.tp:143-169  every (query, train row j ascending)
 //        pair goes through heap_push(dist, j) on a k-slot max-heap initialised to DBL_MAX
 //   sk:utils/_heap.pyx:6-88        heap_push (val >= root rejected; left child preferred on ties)
-//   sk:metrics/_dist_metrics.pxd.tp:39-49  rdist = sum_j (x_j - y_j)^2, j ascending, fp64, no FMA
+//   sk:metrics/_dist_metrics.pxd.tp:39-49  rdist = sum_j (x_j - y_j)^2, j ascending, fp64, no FMA (manhattan: sum_j |x_j - y_j|,
+//        chebyshev: max_j |x_j - y_j|, sk:metrics/_dist_metrics.pyx.tp; the Metric template parameter, rdist in common.h)
 //   sk:neighbors/_classification.py:302  label = mode of the k neighbour classes (lowest class on ties)
 //
 // This kernel is the definition the tensor-core engine (dist_engine.cu) has to reproduce: it is used
@@ -12,7 +13,7 @@
 // query and scans the training rows in index order out of a shared-memory tile (all lanes read the same
 // training row: broadcast), so the heap sees exactly sklearn's push sequence.  Both kernels take the output as a template
 // parameter (KnnOut, common.h): the vote, the distance-weighted vote (weights='distance') or, for kneighbors, the kept rows in
-// ascending (distance, index) order -- the same heap, then knn_finish.
+// ascending (distance, index) order -- the same heap, then knn_finish.  Both are instantiated per metric (Metric, common.h).
 #include <cfloat>
 
 #include "common.h"
@@ -48,7 +49,7 @@ __device__ __forceinline__ void heap_push_dev(double *values, int32_t *indices, 
 
 // OUT == KnnOut::Neighbors (kneighbors) writes nb_ind / nb_dist [n][k] (nb_dist nullable) and leaves labels and proba
 // unused; the votes ignore the two trailing arguments.
-template <typename T, KnnOut OUT>
+template <typename T, Metric M, KnnOut OUT>
 __global__ void __launch_bounds__(kKnnThreads) knn_exact_kernel(const T *__restrict__ X, int64_t n, int d,
                                                                 const double *__restrict__ fit,
                                                                 const int32_t *__restrict__ y, int64_t n_train,
@@ -82,24 +83,26 @@ __global__ void __launch_bounds__(kKnnThreads) knn_exact_kernel(const T *__restr
             if (live) {
                 for (int tt = 0; tt < tn; ++tt) {
                     double dist = 0.0;
-                    for (int j = 0; j < d; ++j) {
-                        double df = __dsub_rn(qs[j * kKnnThreads + tid], ts[tt * d + j]);
-                        dist = __dadd_rn(dist, __dmul_rn(df, df));
-                    }
+                    for (int j = 0; j < d; ++j) dist = rdist<M>(dist, qs[j * kKnnThreads + tid], ts[tt * d + j]);
                     if (dist < hv[0]) heap_push_dev(hv, hi, k, dist, (int32_t)(t0 + tt));
                 }
             }
         }
-        if (live) knn_finish<OUT, 1>(hv, hi, k, C, y, q, labels, proba, nb_ind, nb_dist);
+        if (live) knn_finish<M, OUT, 1>(hv, hi, k, C, y, q, labels, proba, nb_ind, nb_dist);
     }
     if (flag && nf != nf) atomicOr(flag, 1);
 }
 
-template <typename T>
+template <typename T, Metric M>
 static auto exact_kernel(KnnOut out) {
-    return out == KnnOut::Neighbors      ? knn_exact_kernel<T, KnnOut::Neighbors>
-           : out == KnnOut::WeightedVote ? knn_exact_kernel<T, KnnOut::WeightedVote>
-                                         : knn_exact_kernel<T, KnnOut::Vote>;
+    return out == KnnOut::Neighbors      ? knn_exact_kernel<T, M, KnnOut::Neighbors>
+           : out == KnnOut::WeightedVote ? knn_exact_kernel<T, M, KnnOut::WeightedVote>
+                                         : knn_exact_kernel<T, M, KnnOut::Vote>;
+}
+template <typename T>
+static auto exact_kernel(Metric metric, KnnOut out) {
+    return metric == Metric::L1 ? exact_kernel<T, Metric::L1>(out) : metric == Metric::Linf ? exact_kernel<T, Metric::Linf>(out)
+                                                                                          : exact_kernel<T, Metric::L2>(out);
 }
 
 int launch_knn_exact(tcsdn_model *m, const void *x, int64_t n, int dtype, const KnnCall &call, int32_t *flag, cudaStream_t st) {
@@ -111,12 +114,12 @@ int launch_knn_exact(tcsdn_model *m, const void *x, int64_t n, int dtype, const 
     m->stats[0] += 1;
     m->stats[2] += n;
     if (dtype == TCSDN_F32) {
-        auto kern = exact_kernel<float>(call.out);
+        auto kern = exact_kernel<float>(m->knn_metric, call.out);
         TCSDN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kern<<<(unsigned)blocks, kKnnThreads, smem, st>>>(static_cast<const float *>(x), n, m->d, m->d_fit, m->d_y, m->n_train,
                                                           call.k, m->n_classes, call.labels, call.scores, flag, call.ind, call.dist);
     } else {
-        auto kern = exact_kernel<double>(call.out);
+        auto kern = exact_kernel<double>(m->knn_metric, call.out);
         TCSDN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kern<<<(unsigned)blocks, kKnnThreads, smem, st>>>(static_cast<const double *>(x), n, m->d, m->d_fit, m->d_y, m->n_train,
                                                           call.k, m->n_classes, call.labels, call.scores, flag, call.ind, call.dist);
@@ -125,14 +128,14 @@ int launch_knn_exact(tcsdn_model *m, const void *x, int64_t n, int dtype, const 
     return TCSDN_OK;
 }
 
-// The tensor-core engine's tie rows (dist_engine.cu): a few rows per ten thousand whose label depends on which of several
+// The engine's tie rows (dist_engine.cu, both kernels): a few rows per ten thousand whose label depends on which of several
 // equally distant training rows sklearn's index-order heap keeps.  One WARP per row: the lanes compute the distances of 32
 // consecutive training rows (the same rdist arithmetic), and the pushes happen in index order on a heap that every lane keeps
 // in step -- the sequential heap's result at 1/32 of its latency.  The number of rows is only known on the device.
 constexpr int kTieMaxD = 12;   // the engine's feature limit
 
 // lane 0 finishes the row (knn_finish)
-template <typename T, KnnOut OUT>
+template <typename T, Metric M, KnnOut OUT>
 __global__ void __launch_bounds__(256) knn_tie_kernel(const T *__restrict__ X, int d, const double *__restrict__ fit,
                                                       const int32_t *__restrict__ y, int64_t n_train, int k, int C,
                                                       int32_t *__restrict__ labels, double *__restrict__ proba,
@@ -164,10 +167,7 @@ __global__ void __launch_bounds__(256) knn_tie_kernel(const T *__restrict__ X, i
                     double acc = 0.0;
 #pragma unroll
                     for (int j = 0; j < kTieMaxD; ++j)
-                        if (j < d) {
-                            const double df = __dsub_rn(qx[j], fit[t * d + j]);
-                            acc = __dadd_rn(acc, __dmul_rn(df, df));
-                        }
+                        if (j < d) acc = rdist<M>(acc, qx[j], fit[t * d + j]);
                     dist[u] = acc;
                 }
             }
@@ -182,15 +182,20 @@ __global__ void __launch_bounds__(256) knn_tie_kernel(const T *__restrict__ X, i
                 }
             }
         }
-        if (lane == 0) knn_finish<OUT, 1>(hv, hi, k, C, y, q, labels, proba, nb_ind, nb_dist);
+        if (lane == 0) knn_finish<M, OUT, 1>(hv, hi, k, C, y, q, labels, proba, nb_ind, nb_dist);
     }
 }
 
-template <typename T>
+template <typename T, Metric M>
 static auto tie_kernel(KnnOut out) {
-    return out == KnnOut::Neighbors      ? knn_tie_kernel<T, KnnOut::Neighbors>
-           : out == KnnOut::WeightedVote ? knn_tie_kernel<T, KnnOut::WeightedVote>
-                                         : knn_tie_kernel<T, KnnOut::Vote>;
+    return out == KnnOut::Neighbors      ? knn_tie_kernel<T, M, KnnOut::Neighbors>
+           : out == KnnOut::WeightedVote ? knn_tie_kernel<T, M, KnnOut::WeightedVote>
+                                         : knn_tie_kernel<T, M, KnnOut::Vote>;
+}
+template <typename T>
+static auto tie_kernel(Metric metric, KnnOut out) {
+    return metric == Metric::L1 ? tie_kernel<T, Metric::L1>(out) : metric == Metric::Linf ? tie_kernel<T, Metric::Linf>(out)
+                                                                                        : tie_kernel<T, Metric::L2>(out);
 }
 
 int launch_knn_marked(tcsdn_model *m, const void *x, int64_t n, int dtype, const KnnCall &call, const int32_t *list,
@@ -202,11 +207,11 @@ int launch_knn_marked(tcsdn_model *m, const void *x, int64_t n, int dtype, const
     if (blocks > cap) blocks = cap;
     m->stats[0] += 1;
     if (dtype == TCSDN_F32) {
-        auto kern = tie_kernel<float>(call.out);
+        auto kern = tie_kernel<float>(m->knn_metric, call.out);
         kern<<<(unsigned)blocks, 256, 0, st>>>(static_cast<const float *>(x), m->d, m->d_fit, m->d_y, m->n_train, call.k,
                                                m->n_classes, call.labels, call.scores, list, count, total, call.ind, call.dist);
     } else {
-        auto kern = tie_kernel<double>(call.out);
+        auto kern = tie_kernel<double>(m->knn_metric, call.out);
         kern<<<(unsigned)blocks, 256, 0, st>>>(static_cast<const double *>(x), m->d, m->d_fit, m->d_y, m->n_train, call.k,
                                                m->n_classes, call.labels, call.scores, list, count, total, call.ind, call.dist);
     }

@@ -444,8 +444,8 @@ class KMeans(_Base):
 
 
 class KNeighborsClassifier(_Base):
-    """sk:neighbors/_classification.py:245-312 -- k nearest (euclidean, heap order), uniform or distance-weighted vote
-    (``weights='uniform'`` / ``'distance'``; sk:neighbors/_base.py:74-114)."""
+    """sk:neighbors/_classification.py:245-312 -- k nearest (euclidean, manhattan or chebyshev; heap order), uniform or
+    distance-weighted vote (``weights='uniform'`` / ``'distance'``; sk:neighbors/_base.py:74-114)."""
     _kind = "knn"
 
     def __init__(self, n_neighbors=5, **params):
@@ -459,15 +459,21 @@ class KNeighborsClassifier(_Base):
         fx = np.ascontiguousarray(spec["fit_X"], np.float64)
         y = np.ascontiguousarray(spec["y"], np.int32)
         weights = modelio.knn_weights(spec.get("weights", "uniform"))
+        metric = modelio.knn_metric(spec.get("metric", "euclidean"))
         self.n_samples_fit_ = fx.shape[0]
         self.weights = weights
-        _lib.check(lib.tcsdn_knn_create_weighted(_p(fx, _lib._f64p), _p(y, _lib._i32p), fx.shape[0], fx.shape[1],
-                                                 len(spec["classes"]), int(spec["k"]),
-                                                 _lib.KNN_DISTANCE if weights == "distance" else _lib.KNN_UNIFORM, C.byref(h)))
+        self.effective_metric_ = metric
+        args = (_p(fx, _lib._f64p), _p(y, _lib._i32p), fx.shape[0], fx.shape[1], len(spec["classes"]), int(spec["k"]),
+                _lib.KNN_DISTANCE if weights == "distance" else _lib.KNN_UNIFORM)
+        # tcsdn_knn_create_weighted is the euclidean tcsdn_knn_create_metric
+        _lib.check(lib.tcsdn_knn_create_weighted(*args, C.byref(h)) if metric == "euclidean"
+                   else lib.tcsdn_knn_create_metric(*args, _lib.KNN_METRICS[metric], C.byref(h)))
 
     def set_params(self, **params):
         """sklearn applies ``weights`` at predict time, so on a fitted model a new weighting re-creates the handle from the
-        fitted spec (the handle's options, set_option, start from their defaults again)."""
+        fitted spec (the handle's options, set_option, start from their defaults again).  ``metric``, ``p`` and
+        ``metric_params`` are different: sklearn fixes the metric at fit (``effective_metric_``), so on a fitted model they
+        only change the parameters, and the fitted metric stays until the next ``fit``."""
         if "weights" in params and self._spec is not None:
             w = modelio.knn_weights(params["weights"])
             if w != modelio.knn_weights(self._spec.get("weights", "uniform")):
@@ -479,7 +485,7 @@ class KNeighborsClassifier(_Base):
 
     def kneighbors(self, X=None, n_neighbors=None, return_distance=True):
         """sk:neighbors/_base.py:750-960 -- the n_neighbors nearest training rows of every row of X: ``(dist, ind)`` (float64,
-        int64, [n, n_neighbors]), or ``ind`` alone.  The neighbours are the ones ``predict`` votes on (sklearn's index-order
+        int64, [n, n_neighbors]; distances in ``effective_metric_``), or ``ind`` alone.  The neighbours are the ones ``predict`` votes on (sklearn's index-order
         heap); each row is sorted by (distance, training index), where sklearn leaves equal distances in no defined order.
         ``X=None`` queries the training rows and leaves each row's own index out (sklearn's rule).  A CUDA ``torch.Tensor``
         gives CUDA tensors, enqueued on the current stream (``sync_check()`` reports NaN/inf rows).  At most 64 neighbours
@@ -637,6 +643,7 @@ def from_spec(spec):
     if spec["kind"] == "knn":
         est._params["n_neighbors"] = int(spec["k"])
         est._params["weights"] = modelio.knn_weights(spec.get("weights", "uniform"))
+        est._params["metric"] = modelio.knn_metric(spec.get("metric", "euclidean"))
     return est._adopt(spec)
 
 

@@ -19,7 +19,8 @@ linear     coef [R,d] f64, intercept [R] f64, classes  (R == 1 means binary), ov
 gnb        theta [C,d], var [C,d], class_prior [C], classes
 kmeans     centers [k,d]
 knn        fit_X [n_t,d] f64, y [n_t] int32 (class index), k, classes, weights ("uniform" or
-           "distance"; a spec without the key is uniform)
+           "distance"; a spec without the key is uniform), metric ("euclidean", "manhattan" or
+           "chebyshev"; a spec without the key is euclidean)
 svc        sv [nSV,d], dual_coef [C-1,nSV], intercept [P], n_support [C] int32,
            gamma, classes, decision_function_shape, break_ties, kernel ("linear", "poly", "rbf" or
            "sigmoid"; a spec without the key is rbf), coef0, degree
@@ -36,7 +37,7 @@ from typing import Any, Dict
 import numpy as np
 
 __all__ = ["load_reference_pickle", "spec_from_estimator", "spec_from_pickle_bytes",
-           "knn_weights", "svc_kernel", "MODEL_FILES", "SpecError"]
+           "knn_weights", "knn_metric", "svc_kernel", "MODEL_FILES", "SpecError"]
 
 # argv word -> pickle file, as dispatched at reference traffic_classifier.py:229-240
 MODEL_FILES = {
@@ -158,6 +159,38 @@ def knn_weights(w) -> str:
     raise SpecError(f"weights must be 'uniform' or 'distance', got {w!r}")
 
 
+_KNN_METRIC_NAMES = {"euclidean": "euclidean", "l2": "euclidean", "manhattan": "manhattan", "cityblock": "manhattan",
+                     "l1": "manhattan", "chebyshev": "chebyshev", "infinity": "chebyshev"}
+_KNN_MINKOWSKI_P = {1: "manhattan", 2: "euclidean", np.inf: "chebyshev"}
+
+
+def knn_metric(metric, p=2, metric_params=None) -> str:
+    """KNeighborsClassifier's metric as a spec value: "euclidean", "manhattan" or "chebyshev".  Takes scikit-learn's
+    spellings of the three (manhattan = cityblock = l1 = minkowski with p=1, chebyshev = infinity = minkowski with p=inf,
+    euclidean = l2 = minkowski with p=2; ``metric_params`` may hold ``p``, which overrides ``p`` as in scikit-learn).
+    Everything else is refused: minkowski with another p (libm's pow and CUDA's are not bit-identical), weights ``w``,
+    other metrics and callables."""
+    params = {key: v for key, v in dict(metric_params or {}).items() if not (key == "w" and v is None)}
+    supported = "the supported metrics are 'euclidean', 'manhattan' and 'chebyshev'"
+    extra = sorted(set(params) - {"p"})
+    if extra:
+        raise SpecError(f"metric_params {extra} are not implemented; {supported}")
+    if callable(metric) or not isinstance(metric, str):
+        raise SpecError(f"metric {metric!r} is not implemented; {supported}")
+    if metric == "minkowski":
+        p = params.get("p", p)
+        try:
+            name = _KNN_MINKOWSKI_P.get(float(p))
+        except (TypeError, ValueError):
+            name = None
+        if name is None:
+            raise SpecError(f"minkowski with p={p!r} is not implemented; {supported} (minkowski with p=1, 2 or inf)")
+        return name
+    if metric not in _KNN_METRIC_NAMES:
+        raise SpecError(f"metric {metric!r} is not implemented; {supported}")
+    return _KNN_METRIC_NAMES[metric]
+
+
 def svc_kernel(k) -> str:
     """SVC's ``kernel`` as a spec value: one of libsvm's four built-in kernels.  'precomputed' and callables need the
     training rows at predict time and are refused."""
@@ -190,16 +223,17 @@ def _spec_from_attrs(name: str, o) -> Dict[str, Any]:
                     n_features=c.shape[1])
     if name == "KNeighborsClassifier":
         weights = knn_weights(getattr(o, "weights", "uniform"))
-        metric = getattr(o, "effective_metric_", getattr(o, "metric", "minkowski"))
-        p = getattr(o, "p", 2)
-        if not (metric in ("euclidean", "l2") or (metric == "minkowski" and p == 2)):
-            raise SpecError(f"only the euclidean metric is implemented (got {metric}, p={p})")
+        # scikit-learn fixes the metric at fit: effective_metric_ / effective_metric_params_ (sk:neighbors/_base.py:527-552)
+        if hasattr(o, "effective_metric_"):
+            metric = knn_metric(o.effective_metric_, getattr(o, "p", 2), getattr(o, "effective_metric_params_", None))
+        else:
+            metric = knn_metric(getattr(o, "metric", "minkowski"), getattr(o, "p", 2), getattr(o, "metric_params", None))
         fx = _f64(o._fit_X)
         y = np.asarray(o._y)
         if y.ndim != 1:
             raise SpecError("multi-output KNN is not supported")
         return dict(kind="knn", fit_X=fx, y=np.ascontiguousarray(y, dtype=np.int32),
-                    k=int(o.n_neighbors), classes=_classes(o), n_features=fx.shape[1], weights=weights)
+                    k=int(o.n_neighbors), classes=_classes(o), n_features=fx.shape[1], weights=weights, metric=metric)
     if name == "SVC":
         kernel = svc_kernel(getattr(o, "kernel", "rbf"))   # pickles without the attribute are rbf models
         if getattr(o, "_sparse", False):
