@@ -17,8 +17,8 @@ from traffic_classifier_sdn_b200 import _lib, from_spec, synth
 pytestmark = pytest.mark.gpu
 
 SVC_DEC_TOL = 1e-9      # absolute: decision values (fp64 kernel) against libsvm's fp64 (SURVEY 8d policy: <= 1e-5)
-SVC_EPS_MMA = 2.0 ** -19  # csrc/dist_engine.cu kSvcEpsMma
-KAPPA = 2.0 ** -18      # csrc/dist_engine.cu kKappa
+SVC_EPS_MMA = 2.0 ** -19  # csrc/svc_engine.cu kSvcEpsMma
+KAPPA = 2.0 ** -18      # csrc/knn_engine.cu kKappa
 
 
 def _force(est, mode):

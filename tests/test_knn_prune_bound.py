@@ -1,4 +1,4 @@
-"""The KNN engine's pruning rule (csrc/dist_engine.cu, "KNN: spatial order and pruning"), restated in numpy on small data:
+"""The KNN engine's pruning rule (csrc/knn_engine.cu, "KNN: spatial order and pruning"), restated in numpy on small data:
 training rows in kd order -> tiles of 64 with centre and radius; queries sorted by kd leaf -> passes of 256; per pass the
 tiles are visited by centre distance from the home tile and tile t is left out when
 

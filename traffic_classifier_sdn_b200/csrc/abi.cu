@@ -143,8 +143,8 @@ static int run_device(tcsdn_model *m, const void *x, int64_t n, int dtype, int32
         case TCSDN_KIND_KNN: return run_knn(m, x, n, dtype, KnnCall(m, labels, scores), flag, st);
         case TCSDN_KIND_SVC:
             // decision values are always the fp64 kernel's (the engine certifies LABELS; its fp32 sums cannot meet a
-            // 1e-5 absolute bound on decision values, see dist_engine.cu)
-            if (m->opt_engine != 1 && engine_usable(m, n, scores != nullptr)) return launch_svc_engine(m, x, n, dtype, labels, scores, flag, st);
+            // 1e-5 absolute bound on decision values, see svc_engine.cu)
+            if (m->opt_engine != 1 && svc_engine_usable(m, n, scores != nullptr)) return launch_svc_engine(m, x, n, dtype, labels, scores, flag, st);
             // linear kernel: the collapsed label path (svc.cu), certified against the fp64 kernel like the engine
             if (m->opt_engine != 1 && svc_linear_usable(m, scores != nullptr)) return launch_svc_linear(m, x, n, dtype, labels, scores, flag, st);
             if (m->opt_engine >= 2 && !scores) {
@@ -532,7 +532,8 @@ void tcsdn_destroy(tcsdn_model_t *m) {
     int prev = -1;
     cudaGetDevice(&prev);
     cudaSetDevice(m->dev);
-    engine_destroy(m);
+    if (m->kind == TCSDN_KIND_KNN) knn_engine_destroy(m);
+    if (m->kind == TCSDN_KIND_SVC) svc_engine_destroy(m);
     for (Workspace *w : m->pool) free_workspace(w);
     cudaFree(m->d_a); cudaFree(m->d_b); cudaFree(m->d_c);
     cudaFree(m->d_fit); cudaFree(m->d_y);
@@ -585,7 +586,8 @@ int tcsdn_set_option(tcsdn_model_t *m, int32_t key, int64_t value) {
 int tcsdn_model_stats(const tcsdn_model_t *m, int64_t *out) {
     if (!m || !out) { set_error("NULL argument"); return TCSDN_EINVAL; }
     for (int i = 0; i < 8; ++i) out[i] = m->stats[i].load(std::memory_order_relaxed);
-    if (m->engine) engine_read_stats(m, out);   // cumulative since create(); synchronises the device
+    if (m->kind == TCSDN_KIND_KNN) knn_engine_read_stats(m, out);   // engine counters: cumulative since create(); synchronises
+    if (m->kind == TCSDN_KIND_SVC) svc_engine_read_stats(m, out);
     if (m->d_refined) {   // cumulative since create(); synchronises the device
         unsigned long long v = 0;
         if (cudaMemcpy(&v, m->d_refined, sizeof(v), cudaMemcpyDeviceToHost) == cudaSuccess) out[6] = (int64_t)v;

@@ -88,176 +88,19 @@ __device__ __forceinline__ void peer_flag_wait(const GatherOut &G, int which, un
     }
 }
 
-// KNeighborsClassifier's metric, fixed when the handle is created (tcsdn_knn_create_metric).  rdist is what the kernels rank
-// by, in sklearn's arithmetic (sk:metrics/_dist_metrics.pyx.tp, features in order from 0.0, fp64, no FMA):
+// KNeighborsClassifier's metric, fixed when the handle is created (tcsdn_knn_create_metric).  rdist (knn_select.cuh) is what the
+// kernels rank by, in sklearn's arithmetic (sk:metrics/_dist_metrics.pyx.tp, features in order from 0.0, fp64, no FMA):
 //   L2    sum_j (x_j - t_j)^2          (EuclideanDistance.rdist; the distance is its correctly rounded sqrt)
 //   L1    sum_j |x_j - t_j|            (ManhattanDistance.dist)
 //   Linf  max_j |x_j - t_j|            (ChebyshevDistance.dist)
 enum class Metric { L2 = TCSDN_KNN_EUCLIDEAN, L1 = TCSDN_KNN_MANHATTAN, Linf = TCSDN_KNN_CHEBYSHEV };
 
-// the running rdist after one more feature pair (x, t)
-template <Metric M>
-__device__ __forceinline__ double rdist(double acc, double x, double t) {
-    const double df = __dsub_rn(x, t);
-    if constexpr (M == Metric::L2) return __dadd_rn(acc, __dmul_rn(df, df));
-    else if constexpr (M == Metric::L1) return __dadd_rn(acc, fabs(df));
-    else return fmax(acc, fabs(df));
-}
-
-// rdist -> the distance kneighbors reports and distance weights divide by
-template <Metric M>
-__device__ __forceinline__ double to_dist(double r) {
-    if constexpr (M == Metric::L2) return __dsqrt_rn(r);
-    else return r;
-}
-
-// One query's m kept neighbours (rdist, training index), slot i at values[i * ST], sorted in place into the
-// canonical ascending (distance, index) order.  m <= 64: an insertion sort is all it needs.
-template <int ST>
-__device__ __forceinline__ void knn_sort_neighbors(double *values, int32_t *indices, int m) {
-    for (int i = 1; i < m; ++i) {
-        const double v = values[i * ST];
-        const int32_t x = indices[i * ST];
-        int j = i - 1;
-        for (; j >= 0 && (values[j * ST] > v || (values[j * ST] == v && indices[j * ST] > x)); --j) {
-            values[(j + 1) * ST] = values[j * ST];
-            indices[(j + 1) * ST] = indices[j * ST];
-        }
-        values[(j + 1) * ST] = v;
-        indices[(j + 1) * ST] = x;
-    }
-}
-
-// KNeighbors.kneighbors: the neighbours in canonical order, written as one row of ind (and of dist = to_dist<M>, when dist is
-// non-null)
-template <Metric M, int ST>
-__device__ __forceinline__ void knn_write_neighbors(double *values, int32_t *indices, int m, int64_t *ind, double *dist) {
-    knn_sort_neighbors<ST>(values, indices, m);
-    for (int i = 0; i < m; ++i) {
-        ind[i] = indices[i * ST];
-        if (dist) dist[i] = to_dist<M>(values[i * ST]);
-    }
-}
-
-// numpy's float64 row sum (np.sum(a, axis=1), pairwise_sum in numpy/_core/src/umath/loops_utils.h.src) of the n <= 128 terms
-// term(lo) .. term(lo + n - 1): sequential from 0.0 below 8 terms; else eight accumulators seeded with the first eight
-// terms, the following whole groups of 8 added column-wise, the accumulators combined as ((r0+r1)+(r2+r3))+((r4+r5)+(r6+r7)),
-// the remainder added sequentially.  No FMA contraction can change an association: every add is __dadd_rn.
-template <typename F>
-__device__ __forceinline__ double np_sum_block(const F &term, int lo, int n) {
-    if (n < 8) {
-        double res = 0.0;
-        for (int i = 0; i < n; ++i) res = __dadd_rn(res, term(lo + i));
-        return res;
-    }
-    double r[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) r[j] = term(lo + j);
-    int i = 8;
-    for (; i < n - (n % 8); i += 8) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) r[j] = __dadd_rn(r[j], term(lo + i + j));
-    }
-    double res = __dadd_rn(__dadd_rn(__dadd_rn(r[0], r[1]), __dadd_rn(r[2], r[3])), __dadd_rn(__dadd_rn(r[4], r[5]), __dadd_rn(r[6], r[7])));
-    for (; i < n; ++i) res = __dadd_rn(res, term(lo + i));
-    return res;
-}
-
-// the same for n <= 256 terms: above 128 numpy splits at n2 = n/2 - (n/2) % 8 and adds the two halves' sums, recursively
-// (two levels reach 256)
-template <typename F>
-__device__ __forceinline__ double np_sum(const F &term, int n) {
-    auto split = [](int len) { return len / 2 - (len / 2) % 8; };
-    const int nh = n > 128 ? 2 : 1, h0 = nh == 2 ? split(n) : n;
-    double res = 0.0;
-#pragma unroll 1
-    for (int h = 0; h < nh; ++h) {
-        const int lo = h == 0 ? 0 : h0, len = h == 0 ? h0 : n - h0;
-        const int np_ = len > 128 ? 2 : 1, p0 = np_ == 2 ? split(len) : len;
-        double half = 0.0;
-#pragma unroll 1
-        for (int p = 0; p < np_; ++p) {   // (first part) + (second part): the first part is not added to 0.0
-            const double v = np_sum_block(term, p == 0 ? lo : lo + p0, p == 0 ? p0 : len - p0);
-            half = p == 0 ? v : __dadd_rn(half, v);
-        }
-        res = h == 0 ? half : __dadd_rn(res, half);
-    }
-    return res;
-}
-
-// KNeighborsClassifier(weights='distance') for one query (sk:neighbors/_base.py:74-114, _classification.py:281-307,398-410,
-// sk:utils/extmath.py:791-862): values / indices hold the k kept neighbours as (rdist, training index), slot i at
-// [i * ST]; y maps a training index to its class.  The slots are sorted into canonical (distance, index) order and then
-// overwritten with (weight, class):
-//   weight  w_i = 1 / to_dist<M>(d_i), both correctly rounded; if any d_i == 0, w_i = 1 where d_i == 0 and 0 elsewhere
-//   label   per class c, W_c = numpy's row sum (np_sum_block) of the k columns of template_c = (w_i if y_i == c else 0.0);
-//           the lowest class with the largest W_c (weighted_mode: strict > in class order)
-//   proba   (non-null: C entries) P_c = 0.0 + the w_i of class c, sequentially in column order; P_c / (numpy's row sum of
-//           P_0 .. P_{C-1}).  The two sums associate differently, so the label may differ from argmax(proba) in the last
-//           bit exactly as sklearn's may.
-template <Metric M, int ST>
-__device__ __forceinline__ void knn_weighted_vote(double *values, int32_t *indices, int k, int C, const int32_t *__restrict__ y,
-                                                  int32_t *label, double *proba) {
-    knn_sort_neighbors<ST>(values, indices, k);
-    const bool zero = values[0] == 0.0;   // sorted: a zero distance comes first
-    for (int i = 0; i < k; ++i) {
-        const double v = values[i * ST];
-        values[i * ST] = zero ? (v == 0.0 ? 1.0 : 0.0) : __ddiv_rn(1.0, to_dist<M>(v));
-        indices[i * ST] = y[indices[i * ST]];
-    }
-    if (proba)
-        for (int c = 0; c < C; ++c) proba[c] = 0.0;
-    double best = -1.0;
-    int arg = 0;
-    for (int i = 0; i < k; ++i) {   // each class present among the neighbours, at its first column
-        const int32_t c = indices[i * ST];
-        bool seen = false;
-        for (int j = 0; j < i; ++j) seen |= indices[j * ST] == c;
-        if (seen) continue;
-        const double W = np_sum_block([&](int t) { return indices[t * ST] == c ? values[t * ST] : 0.0; }, 0, k);
-        if (W > best || (W == best && c < arg)) { best = W; arg = c; }
-        if (proba) {
-            double p = 0.0;
-            for (int t = i; t < k; ++t)
-                if (indices[t * ST] == c) p = __dadd_rn(p, values[t * ST]);
-            proba[c] = p;
-        }
-    }
-    *label = arg;
-    if (proba) {
-        const double s = np_sum([&](int c) { return proba[c]; }, C);
-        for (int c = 0; c < C; ++c) proba[c] = __ddiv_rn(proba[c], s);
-    }
-}
-
 // What a KNN kernel makes of a query's kept neighbours: the uniform vote (predict), the distance-weighted vote (predict on
 // weights='distance' handles) or the neighbours themselves (kneighbors)
 enum class KnnOut { Vote, WeightedVote, Neighbors };
 
-// Query q's result from its k kept neighbours (values / indices: rdist in metric M and index, slot i at [i * ST]).  y maps an
-// index to its class, so it must match what the indices count: training labels for training indices, the engine's labels in
-// tile order for its tile positions (Vote only: the other two order equal distances by training index).
-//   Vote          labels[q] = the lowest class with the most neighbours; proba (nullable) [n][C] the class fractions
-//   WeightedVote  labels[q] and proba[q] (nullable) from knn_weighted_vote
-//   Neighbors     nb_ind [n][k] the indices and nb_dist [n][k] (nullable) the distances, by knn_write_neighbors
-template <Metric M, KnnOut OUT, int ST>
-__device__ __forceinline__ void knn_finish(double *values, int32_t *indices, int k, int C, const int32_t *__restrict__ y, int64_t q,
-                                           int32_t *labels, double *proba, int64_t *nb_ind, double *nb_dist) {
-    if constexpr (OUT == KnnOut::Neighbors) {
-        knn_write_neighbors<M, ST>(values, indices, k, nb_ind + q * k, nb_dist ? nb_dist + q * k : nullptr);
-    } else if constexpr (OUT == KnnOut::WeightedVote) {
-        knn_weighted_vote<M, ST>(values, indices, k, C, y, labels + q, proba ? proba + q * C : nullptr);
-    } else {
-        int best = 0, arg = 0;
-        for (int c = 0; c < C; ++c) {
-            int votes = 0;
-            for (int i = 0; i < k; ++i) votes += (y[indices[i * ST]] == c);
-            if (proba) proba[q * C + c] = (double)votes / (double)k;
-            if (votes > best) { best = votes; arg = c; }
-        }
-        labels[q] = arg;
-    }
-}
+struct KnnEngine;   // the KNN spatial index and tensor-core operands (knn_engine.cu)
+struct SvcEngine;   // the SVC tensor-core operands (svc_engine.cu)
 
 struct DeviceBuf {
     void *p = nullptr;
@@ -337,7 +180,8 @@ struct tcsdn_model {
     unsigned long long *d_refined = nullptr;   // GaussianNB / linear SVC: rows the certified fast path could not decide (re-run in fp64)
     std::mutex mu;
     std::vector<tcsdn::Workspace *> pool;
-    void *engine = nullptr;          // tensor-core engine state (dist_engine.cu), may be null
+    tcsdn::KnnEngine *knn_engine = nullptr;   // KNN handles: the engine's index and operands, may be null
+    tcsdn::SvcEngine *svc_engine = nullptr;   // SVC handles: the tensor-core engine's operands, may be null
 };
 
 namespace tcsdn {
@@ -379,14 +223,17 @@ int launch_flow_update(double *state, const double *packets, const double *bytes
 int forest_pack(tcsdn_model *m, const int64_t *tree_offsets, const int32_t *left, const int32_t *right,
                 const int32_t *feature, const double *threshold, const double *value, int n_trees, int C);
 
-// tensor-core distance engine (dist_engine.cu).  The create functions build the packed operands; the state is attached to the
-// handle before anything is allocated, so that on an error return tcsdn_destroy frees what was made.
+// tensor-core distance engine (knn_engine.cu, svc_engine.cu).  The create functions build the packed operands; the state is
+// attached to the handle before anything is allocated, so that on an error return tcsdn_destroy frees what was made (the
+// destroy functions).  The read_stats functions write the engine's counters into tcsdn_model_stats's slots (synchronising).
 int knn_engine_create(tcsdn_model *m);
 int svc_engine_create(tcsdn_model *m);
-void engine_destroy(tcsdn_model *m);
-bool engine_usable(const tcsdn_model *m, int64_t n, bool want_scores);
+void knn_engine_destroy(tcsdn_model *m);
+void svc_engine_destroy(tcsdn_model *m);
 bool knn_engine_usable(const tcsdn_model *m, int64_t n, const KnnCall &call);
-void engine_read_stats(const tcsdn_model *m, int64_t *out8);
+bool svc_engine_usable(const tcsdn_model *m, int64_t n, bool want_scores);
+void knn_engine_read_stats(const tcsdn_model *m, int64_t *out8);
+void svc_engine_read_stats(const tcsdn_model *m, int64_t *out8);
 // svc.cu: re-evaluate, in fp64, exactly the rows whose label is negative (-1 - label, left by the engine's certificate);
 // `counter` (device) receives the number of such rows
 int launch_svc_marked(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, unsigned long long *counter,

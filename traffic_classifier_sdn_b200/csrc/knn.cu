@@ -4,48 +4,24 @@
 //        pair goes through heap_push(dist, j) on a k-slot max-heap initialised to DBL_MAX
 //   sk:utils/_heap.pyx:6-88        heap_push (val >= root rejected; left child preferred on ties)
 //   sk:metrics/_dist_metrics.pxd.tp:39-49  rdist = sum_j (x_j - y_j)^2, j ascending, fp64, no FMA (manhattan: sum_j |x_j - y_j|,
-//        chebyshev: max_j |x_j - y_j|, sk:metrics/_dist_metrics.pyx.tp; the Metric template parameter, rdist in common.h)
+//        chebyshev: max_j |x_j - y_j|, sk:metrics/_dist_metrics.pyx.tp; the Metric template parameter, rdist in knn_select.cuh)
 //   sk:neighbors/_classification.py:302  label = mode of the k neighbour classes (lowest class on ties)
 //
-// This kernel is the definition the tensor-core engine (dist_engine.cu) has to reproduce: it is used
+// This kernel is the definition the tensor-core engine (knn_engine.cu) has to reproduce: it is used
 // for small batches (the reference's own call is one row at a time, traffic_classifier.py:106), as the
 // engine's exact re-evaluation rule, and as the engine's cross-check in the tests.  One thread owns one
 // query and scans the training rows in index order out of a shared-memory tile (all lanes read the same
 // training row: broadcast), so the heap sees exactly sklearn's push sequence.  Both kernels take the output as a template
 // parameter (KnnOut, common.h): the vote, the distance-weighted vote (weights='distance') or, for kneighbors, the kept rows in
-// ascending (distance, index) order -- the same heap, then knn_finish.  Both are instantiated per metric (Metric, common.h).
-#include <cfloat>
-
-#include "common.h"
+// ascending (distance, index) order -- the same heap (knn_heap_push), then knn_finish.  Both are instantiated per metric (Metric,
+// common.h).
+#include "knn_select.cuh"
 
 namespace tcsdn {
 
 constexpr int kKnnThreads = 128;
 constexpr int kKnnTile = 128;    // training rows per shared-memory tile
 constexpr int kKnnMaxK = 64;
-
-__device__ __forceinline__ void heap_push_dev(double *values, int32_t *indices, int size, double val, int32_t val_idx) {
-    // caller has already checked val < values[0]
-    values[0] = val;
-    indices[0] = val_idx;
-    int cur = 0;
-    for (;;) {
-        int l = 2 * cur + 1, r = l + 1, swap;
-        if (l >= size) break;
-        if (r >= size) {
-            if (values[l] > val) swap = l; else break;
-        } else if (values[l] >= values[r]) {
-            if (val < values[l]) swap = l; else break;
-        } else {
-            if (val < values[r]) swap = r; else break;
-        }
-        values[cur] = values[swap];
-        indices[cur] = indices[swap];
-        cur = swap;
-    }
-    values[cur] = val;
-    indices[cur] = val_idx;
-}
 
 // OUT == KnnOut::Neighbors (kneighbors) writes nb_ind / nb_dist [n][k] (nb_dist nullable) and leaves labels and proba
 // unused; the votes ignore the two trailing arguments.
@@ -84,7 +60,10 @@ __global__ void __launch_bounds__(kKnnThreads) knn_exact_kernel(const T *__restr
                 for (int tt = 0; tt < tn; ++tt) {
                     double dist = 0.0;
                     for (int j = 0; j < d; ++j) dist = rdist<M>(dist, qs[j * kKnnThreads + tid], ts[tt * d + j]);
-                    if (dist < hv[0]) heap_push_dev(hv, hi, k, dist, (int32_t)(t0 + tt));
+                    if (dist < hv[0]) {   // the push overwrites these root stores; without them ptxas spills the float vote
+                        hv[0] = dist; hi[0] = (int32_t)(t0 + tt);
+                        knn_heap_push<1>(hv, hi, k, dist, (int32_t)(t0 + tt));
+                    }
                 }
             }
         }
@@ -128,7 +107,7 @@ int launch_knn_exact(tcsdn_model *m, const void *x, int64_t n, int dtype, const 
     return TCSDN_OK;
 }
 
-// The engine's tie rows (dist_engine.cu, both kernels): a few rows per ten thousand whose label depends on which of several
+// The engine's tie rows (knn_engine.cu, both kernels): a few rows per ten thousand whose label depends on which of several
 // equally distant training rows sklearn's index-order heap keeps.  One WARP per row: the lanes compute the distances of 32
 // consecutive training rows (the same rdist arithmetic), and the pushes happen in index order on a heap that every lane keeps
 // in step -- the sequential heap's result at 1/32 of its latency.  The number of rows is only known on the device.
@@ -178,7 +157,7 @@ __global__ void __launch_bounds__(256) knn_tie_kernel(const T *__restrict__ X, i
                     const int src = __ffs(m) - 1;
                     m &= m - 1;
                     const double dv = __shfl_sync(0xffffffffu, dist[u], src);
-                    if (dv < root) { heap_push_dev(hv, hi, k, dv, (int32_t)(t0 + 32 * u + src)); root = hv[0]; }
+                    if (dv < root) { knn_heap_push<1>(hv, hi, k, dv, (int32_t)(t0 + 32 * u + src)); root = hv[0]; }
                 }
             }
         }

@@ -285,7 +285,7 @@ __global__ void __launch_bounds__(kThreads) scorer_tiled_kernel(const __grid_con
     float nf = 0.f;
     // Every thread has lifted its rows out of the stage: refill it with the tile kStages rounds ahead.  The bulk copy (async
     // proxy) must not overtake shared loads that are still in flight, and neither BAR.SYNC nor a MEMBAR.CTA in front of it
-    // waits for those (see dist_engine.cu for the hazard): the fp32 pre-pass, whose loaded values are consumed only after the
+    // waits for those (see engine_core.cuh for the hazard): the fp32 pre-pass, whose loaded values are consumed only after the
     // barrier, got rows of the NEXT tile from the refilled stage.  So the barrier's predicate is nf, which depends on every
     // value this thread loaded: the barrier cannot complete before all loads of the CTA have returned.
     auto release = [&](int64_t tile, int stage) {

@@ -75,7 +75,7 @@ __device__ __forceinline__ double svc_kernel_value(double dot, double gamma, dou
 }
 
 // MARKED = false: every row.  MARKED = true: only the rows whose label is negative (the tensor-core engine stores
-// -1 - label for rows its certificate could not decide, dist_engine.cu): a CTA scans a chunk of `chunk` labels, compacts
+// -1 - label for rows its certificate could not decide, svc_engine.cu): a CTA scans a chunk of `chunk` labels, compacts
 // the marked rows' offsets into shared memory and runs the same row-per-thread loop over them, so a support-vector tile
 // staged in shared memory still serves up to 128 rows.
 template <typename T, bool MARKED, int KERNEL>
