@@ -161,6 +161,15 @@ int tcsdn_svc_create_kernel(const double *sv, const double *dual_coef, const dou
                             const int32_t *n_support, int32_t n_sv, int32_t d, int32_t n_classes,
                             int32_t kernel, double gamma, double coef0, int32_t degree, tcsdn_model_t **out);
 
+/* SVC(probability=True): as tcsdn_svc_create_kernel, plus the Platt parameters probA_ / probB_ (prob_a, prob_b
+ * [n_classes*(n_classes-1)/2], copied to HBM) that tcsdn_svc_predict_proba needs.  Both NULL is exactly
+ * tcsdn_svc_create_kernel (engine, collapsed linear path and option rules included); one NULL, or a non-finite value,
+ * returns TCSDN_EINVAL before any device work.  predict and decision values do not depend on them. */
+int tcsdn_svc_create_proba(const double *sv, const double *dual_coef, const double *intercept,
+                           const int32_t *n_support, int32_t n_sv, int32_t d, int32_t n_classes,
+                           int32_t kernel, double gamma, double coef0, int32_t degree,
+                           const double *prob_a, const double *prob_b, tcsdn_model_t **out);
+
 /* RandomForestClassifier: trees concatenated; tree t owns nodes [tree_offsets[t], tree_offsets[t+1]);
  * left/right are node indices local to the tree (-1 = leaf); value [n_nodes][n_classes] are the
  * per-node class fractions DecisionTreeClassifier.predict_proba returns.
@@ -206,6 +215,17 @@ int tcsdn_predict(tcsdn_model_t *m, const void *x, int64_t n, int32_t d, int32_t
  * device pointers set the sticky flag tcsdn_sync_check reads.  Host pointers are processed through the same pipeline as tcsdn_predict. */
 int tcsdn_knn_kneighbors(tcsdn_model_t *m, const void *x, int64_t n, int32_t d, int32_t x_dtype, int32_t x_loc,
                          int32_t n_neighbors, int64_t *ind_out, double *dist_out /* nullable */, void *cuda_stream);
+
+/* SVC.predict_proba(X) (sk:svm/_base.py:867-911; sk:svm/src/libsvm/svm.cpp:2035-2106,2921-2958): per row, libsvm's
+ * Platt sigmoid of each one-vs-one decision value (f = dec * A + B, clamped to [1e-7, 1 - 1e-7]) and its iterative
+ * pairwise coupling (at most max(100, n_classes) rounds, run for two classes too, as scikit-learn does).  proba_out
+ * [n][n_classes] float64 in classes_ order, where x_loc says.  Every operation but exp is an IEEE fp64 operation in libsvm's
+ * order, without FMA.  Always the fp64 kernels (TCSDN_OPT_ENGINE does not apply), in the call that forms the decision
+ * values: no intermediate buffer, no second launch.  TCSDN_EINVAL for a handle that is not an SVC, has no Platt parameters
+ * (tcsdn_svc_create_proba) or gets a bad shape.  Device, counters ([0] kernels, [2] rows) and non-finite rules are
+ * tcsdn_predict's; host pointers go through the same pipeline, device pointers only enqueue on cuda_stream. */
+int tcsdn_svc_predict_proba(tcsdn_model_t *m, const void *x, int64_t n, int32_t d, int32_t x_dtype, int32_t x_loc,
+                            double *proba_out, void *cuda_stream);
 
 /* Host tail of `model.predict`: out[i] = table[idx[i]] for fixed-width class labels (numpy `classes_.take(idx)`,
  * sk:linear_model/_base.py:423), item_bytes bytes per label, gathered on up to n_threads host threads.  Host pointers. */

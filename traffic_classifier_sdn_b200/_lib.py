@@ -47,6 +47,8 @@ SIGNATURES = {
                                    C.POINTER(_vp)]),
     "tcsdn_svc_create_kernel": (C.c_int, [_f64p, _f64p, _f64p, _i32p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_double,
                                           C.c_double, C.c_int32, C.POINTER(_vp)]),
+    "tcsdn_svc_create_proba": (C.c_int, [_f64p, _f64p, _f64p, _i32p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_double,
+                                         C.c_double, C.c_int32, _f64p, _f64p, C.POINTER(_vp)]),
     "tcsdn_forest_create": (C.c_int, [_i64p, _i32p, _i32p, _i32p, _f64p, _f64p, C.c_int32, C.c_int32, C.c_int32,
                                       C.POINTER(_vp)]),
     "tcsdn_destroy": (None, [_vp]),
@@ -56,6 +58,7 @@ SIGNATURES = {
     "tcsdn_set_option": (C.c_int, [_vp, C.c_int32, C.c_int64]),
     "tcsdn_model_stats": (C.c_int, [_vp, _i64p]),
     "tcsdn_predict": (C.c_int, [_vp, _vp, C.c_int64, C.c_int32, C.c_int32, C.c_int32, _vp, _vp, _vp]),
+    "tcsdn_svc_predict_proba": (C.c_int, [_vp, _vp, C.c_int64, C.c_int32, C.c_int32, C.c_int32, _vp, _vp]),
     "tcsdn_knn_kneighbors": (C.c_int, [_vp, _vp, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _vp, _vp, _vp]),
     "tcsdn_take_labels": (C.c_int, [_vp, C.c_int64, _vp, C.c_int32, C.c_int32, _vp, C.c_int32]),
     "tcsdn_sync_check": (C.c_int, [_vp, _vp]),

@@ -509,6 +509,24 @@ int tcsdn_svc_create_kernel(const double *sv, const double *dual_coef, const dou
     return TCSDN_OK;
 }
 
+int tcsdn_svc_create_proba(const double *sv, const double *dual_coef, const double *intercept, const int32_t *n_support,
+                           int32_t n_sv, int32_t d, int32_t n_classes, int32_t kernel, double gamma, double coef0, int32_t degree,
+                           const double *prob_a, const double *prob_b, tcsdn_model_t **out) {
+    if (!prob_a && !prob_b)
+        return tcsdn_svc_create_kernel(sv, dual_coef, intercept, n_support, n_sv, d, n_classes, kernel, gamma, coef0, degree, out);
+    if (out) *out = nullptr;
+    if (!prob_a || !prob_b) { set_error("svc: prob_a and prob_b must both be given or both be NULL"); return TCSDN_EINVAL; }
+    if (n_classes < 2 || n_classes > 16) { set_error("svc: bad arguments (2 <= n_classes <= 16)"); return TCSDN_EINVAL; }
+    const size_t P = (size_t)n_classes * (n_classes - 1) / 2;
+    if (!finite_all(prob_a, P) || !finite_all(prob_b, P)) { set_error("svc: non-finite Platt parameter"); return TCSDN_EINVAL; }
+    TCSDN_TRY(tcsdn_svc_create_kernel(sv, dual_coef, intercept, n_support, n_sv, d, n_classes, kernel, gamma, coef0, degree, out));
+    std::vector<double> platt(prob_a, prob_a + P);
+    platt.insert(platt.end(), prob_b, prob_b + P);
+    const int r = upload(&(*out)->d_platt, platt.data(), platt.size());
+    if (r != TCSDN_OK) { tcsdn_destroy(*out); *out = nullptr; }
+    return r;
+}
+
 int tcsdn_forest_create(const int64_t *tree_offsets, const int32_t *left, const int32_t *right, const int32_t *feature,
                         const double *threshold, const double *value, int32_t n_trees, int32_t d, int32_t n_classes,
                         tcsdn_model_t **out) {
@@ -537,7 +555,7 @@ void tcsdn_destroy(tcsdn_model_t *m) {
     for (Workspace *w : m->pool) free_workspace(w);
     cudaFree(m->d_a); cudaFree(m->d_b); cudaFree(m->d_c);
     cudaFree(m->d_fit); cudaFree(m->d_y);
-    cudaFree(m->d_sv); cudaFree(m->d_coef); cudaFree(m->d_rho); cudaFree(m->d_start); cudaFree(m->d_lin);
+    cudaFree(m->d_sv); cudaFree(m->d_coef); cudaFree(m->d_rho); cudaFree(m->d_start); cudaFree(m->d_lin); cudaFree(m->d_platt);
     cudaFree(m->d_nodes); cudaFree(m->d_tree_base); cudaFree(m->d_group_begin); cudaFree(m->d_leaf_val);
     cudaFree(m->d_flag);
     cudaFree(m->d_refined);
@@ -616,6 +634,28 @@ int tcsdn_predict(tcsdn_model_t *m, const void *x, int64_t n, int32_t d, int32_t
     return run_host(m, x, n, row_bytes, chunk_rows(chunk_bytes, row_bytes), out, out_row, true,
                     [&](const void *xc, int64_t rows, void *labels, void *scores, int32_t *flag, cudaStream_t st) {
                         return run_device(m, xc, rows, x_dtype, static_cast<int32_t *>(labels), static_cast<double *>(scores), flag, st);
+                    });
+}
+
+int tcsdn_svc_predict_proba(tcsdn_model_t *m, const void *x, int64_t n, int32_t d, int32_t x_dtype, int32_t x_loc,
+                            double *proba_out, void *cuda_stream) {
+    if (!m) { set_error("model is NULL"); return TCSDN_EINVAL; }
+    if (m->kind != TCSDN_KIND_SVC) { set_error("predict_proba needs an SVC handle"); return TCSDN_EINVAL; }
+    if (!m->d_platt) { set_error("predict_proba: the SVC handle has no Platt parameters (tcsdn_svc_create_proba)"); return TCSDN_EINVAL; }
+    TCSDN_TRY(check_call(m, x, n, d, x_dtype, x_loc, proba_out, "proba_out"));
+    if (n == 0) return TCSDN_OK;
+    DeviceGuard guard;
+    TCSDN_TRY(begin_call(m, guard));
+    if (x_loc == TCSDN_DEVICE)   // sticky non-finite flag, read by tcsdn_sync_check (as for tcsdn_predict)
+        return launch_svc_proba(m, x, n, x_dtype, proba_out, m->opt_check_finite ? m->d_flag : nullptr,
+                                static_cast<cudaStream_t>(cuda_stream));
+    // the chunking of tcsdn_predict's SVC calls
+    const size_t row_bytes = (size_t)d * (x_dtype == TCSDN_F32 ? 4 : 8);
+    void *const out[2] = {proba_out, nullptr};
+    const size_t out_row[2] = {(size_t)m->n_classes * sizeof(double), 0};
+    return run_host(m, x, n, row_bytes, chunk_rows(128u << 20, row_bytes), out, out_row, true,
+                    [&](const void *xc, int64_t rows, void *proba, void *, int32_t *flag, cudaStream_t st) {
+                        return launch_svc_proba(m, xc, rows, x_dtype, static_cast<double *>(proba), m->opt_check_finite ? flag : nullptr, st);
                     });
 }
 

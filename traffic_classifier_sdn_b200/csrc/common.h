@@ -163,6 +163,7 @@ struct tcsdn_model {
     double coef0 = 0.0;
     int degree = 3;
     double *d_lin = nullptr;     // linear kernel, C <= 8, d <= 16: the collapsed path's parameters (svc.cu), else null
+    double *d_platt = nullptr;   // probability=True models: [2][P], probA_ then probB_ (tcsdn_svc_create_proba), else null
 
     // ---- forest
     uint2 *d_nodes = nullptr;        // packed preorder nodes, all trees
@@ -216,6 +217,8 @@ int launch_knn_marked(tcsdn_model *m, const void *x, int64_t n, int dtype, const
                       const int *count, unsigned long long *total, cudaStream_t st);
 int launch_svc_exact(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, double *scores,
                      int32_t *flag, cudaStream_t st);
+// predict_proba of an SVC handle with Platt parameters: the fp64 kernels' probability mode, proba [n][C] (svc.cu)
+int launch_svc_proba(tcsdn_model *m, const void *x, int64_t n, int dtype, double *proba, int32_t *flag, cudaStream_t st);
 int launch_ovr_from_ovo(const double *dec, int64_t n, int C, double *out, cudaStream_t st);
 int launch_flow_update(double *state, const double *packets, const double *bytes, const double *curr_time,
                        const uint8_t *dir, int64_t n, void *features_out, int feat_dtype, cudaStream_t st);

@@ -22,6 +22,8 @@
 // C-1 running sums of the class being scanned stay in registers and are flushed when the class ends.
 // Two kernels: svc_exact_kernel (any d, up to 16 classes) and svc_exact12_kernel (d <= 12, C <= 8: everything in registers),
 // each templated on the kernel function; the rbf instantiations are the arithmetic this file had before the other kernels.
+// Both have a probability mode (PROBA, predict_proba of probability=True models): the same walk, then libsvm's Platt scaling
+// and pairwise coupling per row (svc_proba.cuh) in place of the vote; the other instantiations are unchanged by it.
 //
 // Collapsed linear labels (svc_linear_kernel).  A linear model's decision values are dec_p = W_p . x - rho_p with
 // W_p = sum_{s in pair p} c_ps sv_s (c_ps: the coefficient above), so a label needs P x d fp64 FMAs per row instead of a
@@ -48,6 +50,7 @@
 #include <cmath>
 
 #include "common.h"
+#include "svc_proba.cuh"
 
 namespace tcsdn {
 
@@ -78,7 +81,10 @@ __device__ __forceinline__ double svc_kernel_value(double dot, double gamma, dou
 // -1 - label for rows its certificate could not decide, svc_engine.cu): a CTA scans a chunk of `chunk` labels, compacts
 // the marked rows' offsets into shared memory and runs the same row-per-thread loop over them, so a support-vector tile
 // staged in shared memory still serves up to 128 rows.
-template <typename T, bool MARKED, int KERNEL>
+// PROBA = true (MARKED = false only): no labels and no decision values; once a row's decision values are complete the
+// thread turns them into the C probabilities of predict_proba (svc_proba.cuh) and writes them to proba_out [n][C].
+// platt [2][P]: probA_, then probB_.
+template <typename T, bool MARKED, int KERNEL, bool PROBA>
 __global__ void __launch_bounds__(kSvcThreads) svc_exact_kernel(const T *__restrict__ X, int64_t n, int d,
                                                                 const double *__restrict__ sv,
                                                                 const double *__restrict__ coef,
@@ -86,7 +92,9 @@ __global__ void __launch_bounds__(kSvcThreads) svc_exact_kernel(const T *__restr
                                                                 const int32_t *__restrict__ start, int n_sv, int C,
                                                                 double gamma, int32_t *__restrict__ labels,
                                                                 double *__restrict__ dec_out, int32_t *flag, int chunk,
-                                                                unsigned long long *counter, double coef0, int degree) {
+                                                                unsigned long long *counter, double coef0, int degree,
+                                                                const double *__restrict__ platt,
+                                                                double *__restrict__ proba_out) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     double *xs = reinterpret_cast<double *>(smem_raw);       // [d][kSvcThreads]
     double *ss = xs + (size_t)d * kSvcThreads;               // [kSvcTile][d]
@@ -171,6 +179,15 @@ __global__ void __launch_bounds__(kSvcThreads) svc_exact_kernel(const T *__restr
                     if (mm < Cm1) { S[ci * Cm1 + mm] = acc[mm]; acc[mm] = 0.0; }
                 ++ci;
             }
+            if constexpr (PROBA) {
+                double v[kSvcMaxC * (kSvcMaxC - 1) / 2];
+                const int P = C * (C - 1) / 2;
+                int p = 0;
+                for (int i = 0; i < C; ++i)
+                    for (int j = i + 1; j < C; ++j, ++p) v[p] = (S[i * Cm1 + (j - 1)] + S[j * Cm1 + i]) - rho[p];
+                svc_proba_row<kSvcMaxC>(C, v, platt, platt + P, proba_out + row * C);
+                continue;
+            }
             int vote[kSvcMaxC];
             for (int c = 0; c < C; ++c) vote[c] = 0;
             int p = 0;
@@ -197,7 +214,7 @@ __global__ void __launch_bounds__(kSvcThreads) svc_exact_kernel(const T *__restr
 // the C-1 running sums and the C(C-1)/2 decision values stay in registers (no local memory: the generic kernel above keeps
 // S[16][15] on the stack).  Per pair: 24 fp64 operations for the distance, exp(), C-1 DFMA -- bound by the fp64 pipe, not
 // by shared-memory loads (the generic kernel issues 29 of them per pair).  Summation order as in the generic kernel.
-template <typename T, bool MARKED, int C, int KERNEL>
+template <typename T, bool MARKED, int C, int KERNEL, bool PROBA>
 __global__ void __launch_bounds__(kSvcThreads) svc_exact12_kernel(const T *__restrict__ X, int64_t n, int d,
                                                                   const double *__restrict__ sv,
                                                                   const double *__restrict__ coef,
@@ -205,7 +222,8 @@ __global__ void __launch_bounds__(kSvcThreads) svc_exact12_kernel(const T *__res
                                                                   const int32_t *__restrict__ start, int n_sv, double gamma,
                                                                   int32_t *__restrict__ labels, double *__restrict__ dec_out,
                                                                   int32_t *flag, int chunk, unsigned long long *counter,
-                                                                  double coef0, int degree) {
+                                                                  double coef0, int degree, const double *__restrict__ platt,
+                                                                  double *__restrict__ proba_out) {
     constexpr int D = 12, Cm1 = C - 1, P = C * (C - 1) / 2;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     double *ss = reinterpret_cast<double *>(smem_raw);            // [kSvcTile][D]
@@ -316,7 +334,12 @@ __global__ void __launch_bounds__(kSvcThreads) svc_exact12_kernel(const T *__res
                     dec[i * C - (i * (i + 1)) / 2 + (jj - i - 1)] += acc[mm];
                 }
             }
-            if (live) {
+            if (live && PROBA) {
+                double v[P];
+#pragma unroll
+                for (int p = 0; p < P; ++p) v[p] = dec[p] - rho[p];
+                svc_proba_row<C>(C, v, platt, platt + P, proba_out + row * C);
+            } else if (live) {
                 int vote[C];
 #pragma unroll
                 for (int c = 0; c < C; ++c) vote[c] = 0;
@@ -370,19 +393,21 @@ int launch_ovr_from_ovo(const double *dec, int64_t n, int C, double *out, cudaSt
     return TCSDN_OK;
 }
 
-template <typename T, bool MARKED, int C, int KERNEL>
+// PROBA: `scores` is the probability output [n][C] (no labels, no decision values)
+template <typename T, bool MARKED, int C, int KERNEL, bool PROBA>
 static int launch_svc12(tcsdn_model *m, const T *x, int64_t n, int32_t *labels, double *scores, int32_t *flag,
                         unsigned long long *counter, int chunk, int64_t blocks, cudaStream_t st) {
-    auto kern = svc_exact12_kernel<T, MARKED, C, KERNEL>;
+    auto kern = svc_exact12_kernel<T, MARKED, C, KERNEL, PROBA>;
     const size_t smem = (size_t)kSvcTile * (12 + 8) * sizeof(double) + (MARKED ? (size_t)chunk * sizeof(uint16_t) : 0);
     TCSDN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     kern<<<(unsigned)blocks, kSvcThreads, smem, st>>>(x, n, m->d, m->d_sv, m->d_coef, m->d_rho, m->d_start, m->n_sv, m->gamma,
-                                                      labels, scores, flag, chunk, counter, m->coef0, m->degree);
+                                                      labels, PROBA ? nullptr : scores, flag, chunk, counter, m->coef0, m->degree,
+                                                      PROBA ? m->d_platt : nullptr, PROBA ? scores : nullptr);
     TCSDN_CUDA(cudaGetLastError());
     return TCSDN_OK;
 }
 
-template <typename T, bool MARKED, int KERNEL>
+template <typename T, bool MARKED, int KERNEL, bool PROBA>
 static int launch_svc_t(tcsdn_model *m, const T *x, int64_t n, int32_t *labels, double *scores, int32_t *flag,
                         unsigned long long *counter, cudaStream_t st) {
     if (m->n_classes > kSvcMaxC) { set_error("svc: more than %d classes", kSvcMaxC); return TCSDN_EINVAL; }
@@ -400,32 +425,33 @@ static int launch_svc_t(tcsdn_model *m, const T *x, int64_t n, int32_t *labels, 
     m->stats[0] += 1;
     if (m->d <= 12 && m->n_classes <= 8) {
         switch (m->n_classes) {
-#define TCSDN_CASE(CC) case CC: return launch_svc12<T, MARKED, CC, KERNEL>(m, x, n, labels, scores, flag, counter, chunk, blocks, st);
+#define TCSDN_CASE(CC) case CC: return launch_svc12<T, MARKED, CC, KERNEL, PROBA>(m, x, n, labels, scores, flag, counter, chunk, blocks, st);
             TCSDN_CASE(2) TCSDN_CASE(3) TCSDN_CASE(4) TCSDN_CASE(5) TCSDN_CASE(6) TCSDN_CASE(7) TCSDN_CASE(8)
 #undef TCSDN_CASE
         }
     }
     const size_t smem = ((size_t)m->d * kSvcThreads + (size_t)kSvcTile * m->d + (size_t)(m->n_classes - 1) * kSvcTile) *
                         sizeof(double) + (MARKED ? (size_t)chunk * sizeof(uint16_t) : 0);
-    auto kern = svc_exact_kernel<T, MARKED, KERNEL>;
+    auto kern = svc_exact_kernel<T, MARKED, KERNEL, PROBA>;
     TCSDN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     kern<<<(unsigned)blocks, kSvcThreads, smem, st>>>(x, n, m->d, m->d_sv, m->d_coef, m->d_rho, m->d_start, m->n_sv, m->n_classes,
-                                                      m->gamma, labels, scores, flag, chunk, counter, m->coef0, m->degree);
+                                                      m->gamma, labels, PROBA ? nullptr : scores, flag, chunk, counter, m->coef0,
+                                                      m->degree, PROBA ? m->d_platt : nullptr, PROBA ? scores : nullptr);
     TCSDN_CUDA(cudaGetLastError());
     return TCSDN_OK;
 }
 
-template <typename T, bool MARKED>
+template <typename T, bool MARKED, bool PROBA = false>
 static int launch_svc_k(tcsdn_model *m, const T *x, int64_t n, int32_t *labels, double *scores, int32_t *flag,
                         unsigned long long *counter, cudaStream_t st) {
     // marked rows come from the rbf engine or the linear collapsed path only: poly / sigmoid have no MARKED instantiation
     switch (m->svc_kernel) {
-        case TCSDN_SVC_RBF: return launch_svc_t<T, MARKED, TCSDN_SVC_RBF>(m, x, n, labels, scores, flag, counter, st);
-        case TCSDN_SVC_LINEAR: return launch_svc_t<T, MARKED, TCSDN_SVC_LINEAR>(m, x, n, labels, scores, flag, counter, st);
+        case TCSDN_SVC_RBF: return launch_svc_t<T, MARKED, TCSDN_SVC_RBF, PROBA>(m, x, n, labels, scores, flag, counter, st);
+        case TCSDN_SVC_LINEAR: return launch_svc_t<T, MARKED, TCSDN_SVC_LINEAR, PROBA>(m, x, n, labels, scores, flag, counter, st);
         default:
             if constexpr (!MARKED) {
-                if (m->svc_kernel == TCSDN_SVC_POLY) return launch_svc_t<T, false, TCSDN_SVC_POLY>(m, x, n, labels, scores, flag, counter, st);
-                return launch_svc_t<T, false, TCSDN_SVC_SIGMOID>(m, x, n, labels, scores, flag, counter, st);
+                if (m->svc_kernel == TCSDN_SVC_POLY) return launch_svc_t<T, false, TCSDN_SVC_POLY, PROBA>(m, x, n, labels, scores, flag, counter, st);
+                return launch_svc_t<T, false, TCSDN_SVC_SIGMOID, PROBA>(m, x, n, labels, scores, flag, counter, st);
             }
     }
     set_error("svc: no marked-row re-evaluation for kernel %d", m->svc_kernel);
@@ -450,6 +476,13 @@ int launch_svc_marked(tcsdn_model *m, const void *x, int64_t n, int dtype, int32
                       cudaStream_t st) {
     if (n == 0) return TCSDN_OK;
     return launch_svc_impl<true>(m, x, n, dtype, labels, nullptr, nullptr, counter, st);
+}
+
+int launch_svc_proba(tcsdn_model *m, const void *x, int64_t n, int dtype, double *proba, int32_t *flag, cudaStream_t st) {
+    if (n == 0) return TCSDN_OK;
+    m->stats[2] += n;
+    if (dtype == TCSDN_F32) return launch_svc_k<float, false, true>(m, static_cast<const float *>(x), n, nullptr, proba, flag, nullptr, st);
+    return launch_svc_k<double, false, true>(m, static_cast<const double *>(x), n, nullptr, proba, flag, nullptr, st);
 }
 
 // ---- collapsed linear labels (derivation in the file header)

@@ -6,7 +6,7 @@ These classes are the drop-in for the objects the reference gets from ``pickle.l
 
 * ``fit(X, y=None) -> self``; ``predict(X) -> ndarray[n]`` of ``classes_`` dtype (int32 cluster ids for
   KMeans); ``classes_``, ``n_features_in_``; ``decision_function`` (LogisticRegression, SVC),
-  ``predict_proba`` (GaussianNB, KNeighborsClassifier, RandomForestClassifier), ``predict_log_proba`` /
+  ``predict_proba`` (GaussianNB, KNeighborsClassifier, RandomForestClassifier, SVC(probability=True)), ``predict_log_proba`` /
   ``transform`` where sklearn has them and they are a closed form of the kernel's score matrix;
   ``kneighbors`` (KNeighborsClassifier);
 * ``ValueError`` on a wrong feature count or NaN/inf input, ``NotFittedError`` before ``fit``;
@@ -551,7 +551,14 @@ class SVC(_Base):
         self.break_ties = bool(spec.get("break_ties", False))
         self.kernel = modelio.svc_kernel(spec.get("kernel", "rbf"))
         self.coef0, self.degree = float(spec.get("coef0", 0.0)), int(spec.get("degree", 3))
-        if self.kernel == "rbf":
+        self._platt = modelio.svc_platt(spec.get("prob_a"), spec.get("prob_b"), len(nsup))
+        if self._platt is not None:   # probability=True: the same handle plus probA_ / probB_ in HBM
+            f = _lib._f64p
+            _lib.check(lib.tcsdn_svc_create_proba(_p(sv, f), _p(dual, f), _p(icpt, f), _p(nsup, _lib._i32p), sv.shape[0],
+                                                  sv.shape[1], len(nsup), _lib.SVC_KERNELS[self.kernel], float(spec["gamma"]),
+                                                  self.coef0, self.degree, _p(self._platt[0], f), _p(self._platt[1], f),
+                                                  C.byref(h)))
+        elif self.kernel == "rbf":
             _lib.check(lib.tcsdn_svc_create(_p(sv, _lib._f64p), _p(dual, _lib._f64p), _p(icpt, _lib._f64p),
                                             _p(nsup, _lib._i32p), sv.shape[0], sv.shape[1], len(nsup),
                                             float(spec["gamma"]), C.byref(h)))
@@ -581,6 +588,60 @@ class SVC(_Base):
             coef = np.vstack(rows)
         coef.flags.writeable = False
         return coef
+
+    def _platt_array(self, i):
+        self._check_fitted()
+        a = np.zeros(0) if self._platt is None else self._platt[i].copy()
+        a.flags.writeable = False
+        return a
+
+    @property
+    def probA_(self):
+        """Platt scaling parameter A per class pair (empty unless fitted with probability=True).  Read-only, as in sklearn."""
+        return self._platt_array(0)
+
+    @property
+    def probB_(self):
+        """Platt scaling parameter B per class pair (empty unless fitted with probability=True).  Read-only, as in sklearn."""
+        return self._platt_array(1)
+
+    def _check_proba(self):
+        """sk:svm/_base.py _check_proba: predict_proba / predict_log_proba exist only for probability=True (or an imported
+        model that carries Platt parameters); hasattr() is False otherwise."""
+        if not (self._params.get("probability", False) or getattr(self, "_platt", None) is not None):
+            raise AttributeError("predict_proba is not available when probability=False")
+        return True
+
+    @property
+    def predict_proba(self):
+        """sk:svm/_base.py:867-911 -- libsvm's Platt sigmoid per class pair and pairwise coupling, on the GPU
+        (tcsdn_svc_predict_proba): [n, n_classes] float64 in ``classes_`` order.  ``predict`` stays libsvm's vote, which can
+        differ from the argmax of these probabilities, as in sklearn.  A CUDA ``torch.Tensor`` gives a CUDA tensor,
+        enqueued on the current stream (``sync_check()`` reports NaN/inf rows)."""
+        self._check_proba()
+        return self._predict_proba
+
+    @property
+    def predict_log_proba(self):
+        """log(predict_proba(X)): ``np.log`` for numpy rows, ``torch.log`` for CUDA tensors."""
+        self._check_proba()
+        return self._predict_log_proba
+
+    def _predict_proba(self, X):
+        self._check_fitted()
+        if self._platt is None:
+            raise NotFittedError("predict_proba is not available when fitted with probability=False")
+        X, n, d, dt, loc = _rows(X)
+        lib = _lib.load()
+        return _call(X, loc, [((n, len(self.classes_)), np.float64)],
+                     lambda x, o, st: lib.tcsdn_svc_predict_proba(self._handle, x, n, d, dt, loc, o[0], st))[0]
+
+    def _predict_log_proba(self, X):
+        p = self._predict_proba(X)
+        if isinstance(p, np.ndarray):
+            return np.log(p)
+        import torch
+        return torch.log(p)
 
     def _ovo(self, X):
         return self._scores(X)
@@ -644,6 +705,8 @@ def from_spec(spec):
         est._params["n_neighbors"] = int(spec["k"])
         est._params["weights"] = modelio.knn_weights(spec.get("weights", "uniform"))
         est._params["metric"] = modelio.knn_metric(spec.get("metric", "euclidean"))
+    if spec["kind"] == "svc" and spec.get("prob_a") is not None and np.asarray(spec["prob_a"]).size:
+        est._params["probability"] = True
     return est._adopt(spec)
 
 

@@ -23,7 +23,8 @@ knn        fit_X [n_t,d] f64, y [n_t] int32 (class index), k, classes, weights (
            "chebyshev"; a spec without the key is euclidean)
 svc        sv [nSV,d], dual_coef [C-1,nSV], intercept [P], n_support [C] int32,
            gamma, classes, decision_function_shape, break_ties, kernel ("linear", "poly", "rbf" or
-           "sigmoid"; a spec without the key is rbf), coef0, degree
+           "sigmoid"; a spec without the key is rbf), coef0, degree, prob_a / prob_b [P] f64 (probA_ /
+           probB_: the Platt parameters of a probability=True model; absent for other models)
 forest     tree_offsets [T+1] int64, left/right/feature int32 [N], threshold f64 [N],
            value [N,C] f64 (per-node class fractions), classes
 =========  ==========================================================================
@@ -37,7 +38,7 @@ from typing import Any, Dict
 import numpy as np
 
 __all__ = ["load_reference_pickle", "spec_from_estimator", "spec_from_pickle_bytes",
-           "knn_weights", "knn_metric", "svc_kernel", "MODEL_FILES", "SpecError"]
+           "knn_weights", "knn_metric", "svc_kernel", "svc_platt", "MODEL_FILES", "SpecError"]
 
 # argv word -> pickle file, as dispatched at reference traffic_classifier.py:229-240
 MODEL_FILES = {
@@ -201,6 +202,21 @@ def svc_kernel(k) -> str:
     raise SpecError(f"kernel must be 'linear', 'poly', 'rbf' or 'sigmoid', got {k!r}")
 
 
+def svc_platt(prob_a, prob_b, n_classes):
+    """SVC's Platt parameters (probA_, probB_) as spec values: None when both are missing or empty (a model fitted with
+    probability=False), else two contiguous float64 arrays of n_classes * (n_classes - 1) / 2 finite values."""
+    a = np.zeros(0) if prob_a is None else np.asarray(prob_a, dtype=np.float64).ravel()
+    b = np.zeros(0) if prob_b is None else np.asarray(prob_b, dtype=np.float64).ravel()
+    if a.size == 0 and b.size == 0:
+        return None
+    P = n_classes * (n_classes - 1) // 2
+    if a.size != P or b.size != P:
+        raise SpecError(f"probA_ / probB_ must hold {P} values each (one per class pair), got {a.size} and {b.size}")
+    if not (np.isfinite(a).all() and np.isfinite(b).all()):
+        raise SpecError("probA_ / probB_ must be finite")
+    return np.ascontiguousarray(a), np.ascontiguousarray(b)
+
+
 def _spec_from_attrs(name: str, o) -> Dict[str, Any]:
     if name == "LogisticRegression":
         coef = _f64(o.coef_)
@@ -246,11 +262,20 @@ def _spec_from_attrs(name: str, o) -> Dict[str, Any]:
         dual = _f64(getattr(o, "_dual_coef_", o.dual_coef_))
         icpt = _f64(getattr(o, "_intercept_", o.intercept_))
         nsup = np.asarray(getattr(o, "_n_support", getattr(o, "n_support_", None)), dtype=np.int32)
-        return dict(kind="svc", sv=sv, dual_coef=dual, intercept=icpt, n_support=np.ascontiguousarray(nsup),
+        spec = dict(kind="svc", sv=sv, dual_coef=dual, intercept=icpt, n_support=np.ascontiguousarray(nsup),
                     gamma=float(o._gamma), classes=cls, n_features=sv.shape[1],
                     decision_function_shape=str(o.decision_function_shape),
                     break_ties=bool(getattr(o, "break_ties", False)), n_classes=C, kernel=kernel,
                     coef0=float(getattr(o, "coef0", 0.0)), degree=int(getattr(o, "degree", 3)))
+        # Platt parameters of a probability=True fit (sk:svm/_base.py: _probA / _probB, public as probA_ / probB_)
+        # (the private names first: scikit-learn 1.9 warns on every read of the deprecated public ones)
+        pa, pb = getattr(o, "_probA", None), getattr(o, "_probB", None)
+        if pa is None and pb is None:
+            pa, pb = getattr(o, "probA_", None), getattr(o, "probB_", None)
+        platt = svc_platt(pa, pb, C)
+        if platt is not None:
+            spec["prob_a"], spec["prob_b"] = platt
+        return spec
     if name == "RandomForestClassifier":
         cls = _classes(o)
         if cls is None or (len(cls) and isinstance(cls[0], np.ndarray)):
