@@ -227,6 +227,23 @@ int tcsdn_knn_kneighbors(tcsdn_model_t *m, const void *x, int64_t n, int32_t d, 
 int tcsdn_svc_predict_proba(tcsdn_model_t *m, const void *x, int64_t n, int32_t d, int32_t x_dtype, int32_t x_loc,
                             double *proba_out, void *cuda_stream);
 
+/* KMeans.transform(X) and KMeans.score(X) (sk:cluster/_kmeans.py: transform, score) on a KMeans handle; TCSDN_EINVAL for any
+ * other kind.  Both use one squared distance, scikit-learn's _euclidean_dense_dense (sk:cluster/_k_means_common.pyx:16-43):
+ * the features in groups of four, ((d0 d0 + d1 d1) + d2 d2) + d3 d3 per group with d_j = x_j - c_j, added to the running
+ * result, then the remaining features one at a time; fp64, no FMA; float32 rows are widened first.
+ *   tcsdn_kmeans_transform  dist_out [n][k] float64, where x_loc says: the correctly rounded sqrt of that distance to every
+ *                           centre.
+ *   tcsdn_kmeans_score      *inertia_out (a HOST double) = the sum over the rows of the distance to the row's centre, where
+ *                           the centre is predict's label (||c||^2 - 2 x.c, first minimum).  Per-CTA partial sums are added in a
+ *                           fixed order: the same call returns the same bits.  The call returns when the sum is on the host;
+ *                           n = 0 gives 0.
+ * Device, counters ([0] kernels) and non-finite rules are tcsdn_predict's: host pointers go through the same pipeline and
+ * return TCSDN_ENONFINITE, device pointers set the sticky flag tcsdn_sync_check reads. */
+int tcsdn_kmeans_transform(tcsdn_model_t *m, const void *x, int64_t n, int32_t d, int32_t x_dtype, int32_t x_loc,
+                           double *dist_out, void *cuda_stream);
+int tcsdn_kmeans_score(tcsdn_model_t *m, const void *x, int64_t n, int32_t d, int32_t x_dtype, int32_t x_loc,
+                       double *inertia_out /* host */, void *cuda_stream);
+
 /* Host tail of `model.predict`: out[i] = table[idx[i]] for fixed-width class labels (numpy `classes_.take(idx)`,
  * sk:linear_model/_base.py:423), item_bytes bytes per label, gathered on up to n_threads host threads.  Host pointers. */
 int tcsdn_take_labels(const int32_t *idx, int64_t n, const void *table, int32_t n_items, int32_t item_bytes, void *out,
@@ -264,6 +281,22 @@ int tcsdn_gnb_fit(const void *x, const int32_t *y, int64_t n, int32_t d, int32_t
 int tcsdn_kmeans_fit(const void *x, int64_t n, int32_t d, int32_t k, int32_t x_dtype, int32_t loc,
                      const double *init_centers, int32_t max_iter, double tol, double *centers_out,
                      int32_t *labels_out, double *inertia_out, int32_t *n_iter_out, void *cuda_stream);
+
+/* tcsdn_kmeans_plusplus  k-means++ seeding, sklearn.cluster.kmeans_plusplus with unit sample weights
+ *                   (sk:cluster/_kmeans.py:_kmeans_plusplus) on the rows as given (not mean-centred), without a host copy of
+ *                   device rows.  The caller draws the random numbers in scikit-learn's order: first_index =
+ *                   rs.choice(n, p=ones(n) / n), then for each later centre rs.uniform(size=n_local_trials), concatenated in
+ *                   uniforms [(k - 1) * n_local_trials] (HOST; may be NULL for k = 1).  Per centre, candidate l is the first
+ *                   row whose prefix sum of the closest squared distances (kmeans_dist: tcsdn_kmeans_transform's distance)
+ *                   reaches uniforms_l * potential (clipped to n - 1; row 0 when the potential is 0), and the candidate with
+ *                   the smallest new potential (first minimum) becomes the centre.  Sums follow one fixed tree (kmeanspp.cu):
+ *                   the same arguments give the same centres.  indices_out [k] int64 and centers_out [k][d] float64 (the
+ *                   chosen rows, widened) are HOST arrays, complete when the call returns.  1 <= k <= n, n_local_trials >= 1,
+ *                   0 <= first_index < n; TCSDN_EINVAL otherwise or for a NULL pointer, before any device work;
+ *                   TCSDN_ENONFINITE for NaN / inf rows.  Host rows are copied to the device once. */
+int tcsdn_kmeans_plusplus(const void *x, int64_t n, int32_t d, int32_t k, int32_t x_dtype, int32_t loc, int64_t first_index,
+                          int32_t n_local_trials, const double *uniforms, int64_t *indices_out, double *centers_out,
+                          void *cuda_stream);
 
 /* ---- multi-GPU (SURVEY 8e): one process per GPU, rows sharded, models replicated ------------------
  * predict() never communicates: rank r classifies its contiguous block of n_block = ceil(n / world) rows.  The only

@@ -9,7 +9,7 @@ six scikit-learn estimators, with hand-written CUDA kernels behind a C ABI (``in
     labels = model.predict(rows)                           # runs on the GPU; no CPU fallback exists
 """
 from .estimators import (GaussianNB, KMeans, KNeighborsClassifier, LogisticRegression, NotFittedError,  # noqa: F401
-                         RandomForestClassifier, SVC, from_sklearn, from_spec, load_model)
+                         RandomForestClassifier, SVC, from_sklearn, from_spec, kmeans_plusplus, load_model)
 from .modelio import MODEL_FILES, load_reference_pickle, spec_from_estimator  # noqa: F401
 
 __version__ = "0.1.0"

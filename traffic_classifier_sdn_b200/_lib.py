@@ -68,6 +68,10 @@ SIGNATURES = {
                                 _f64p, _f64p, _f64p, _vp]),
     "tcsdn_kmeans_fit": (C.c_int, [_vp, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _f64p, C.c_int32, C.c_double,
                                    _f64p, _vp, _f64p, _i32p, _vp]),
+    "tcsdn_kmeans_transform": (C.c_int, [_vp, _vp, C.c_int64, C.c_int32, C.c_int32, C.c_int32, _vp, _vp]),
+    "tcsdn_kmeans_score": (C.c_int, [_vp, _vp, C.c_int64, C.c_int32, C.c_int32, C.c_int32, _f64p, _vp]),
+    "tcsdn_kmeans_plusplus": (C.c_int, [_vp, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int64, C.c_int32, _f64p,
+                                        _i64p, _f64p, _vp]),
     "tcsdn_comm_unique_id": (C.c_int, [_vp]),
     "tcsdn_comm_init": (C.c_int, [C.c_int32, C.c_int32, _vp, C.POINTER(_vp)]),
     "tcsdn_allgather_labels": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, _vp, _vp]),

@@ -209,7 +209,7 @@ static int run_host(tcsdn_model *m, const void *x, int64_t n, size_t row_bytes, 
                     const size_t out_row[2], bool stage_pageable, const Launch &launch) {
     if (m->opt_chunk_rows > 0) chunk = m->opt_chunk_rows;
     if (chunk > n) chunk = n;
-    const int n_out = out[1] ? 2 : 1;
+    const int n_out = out[0] ? (out[1] ? 2 : 1) : 0;   // no per-row output: a reduction (tcsdn_kmeans_score)
     auto is_pinned = [](const void *p) {
         cudaPointerAttributes a;
         if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
@@ -400,8 +400,9 @@ int tcsdn_kmeans_create(const double *centers, int32_t k, int32_t d, tcsdn_model
     if (!finite_all(centers, (size_t)k * d)) { set_error("kmeans: non-finite center"); return TCSDN_EINVAL; }
     tcsdn_model *m;
     TCSDN_TRY(model_base(&m, TCSDN_KIND_KMEANS, d, k, k));
-    // score_j = ||c_j||^2 - 2 x.c_j, argmin  (sk:cluster/_k_means_lloyd.pyx:191-213)
-    std::vector<double> a((size_t)k * d), b((size_t)k * d, 0.0), c(k);
+    // score_j = ||c_j||^2 - 2 x.c_j, argmin  (sk:cluster/_k_means_lloyd.pyx:191-213); b holds the centres themselves, for
+    // transform and score (the argmin does not read it)
+    std::vector<double> a((size_t)k * d), b(centers, centers + (size_t)k * d), c(k);
     for (int i = 0; i < k; ++i) {
         double s = 0.0;
         for (int j = 0; j < d; ++j) {
@@ -657,6 +658,80 @@ int tcsdn_svc_predict_proba(tcsdn_model_t *m, const void *x, int64_t n, int32_t 
                     [&](const void *xc, int64_t rows, void *proba, void *, int32_t *flag, cudaStream_t st) {
                         return launch_svc_proba(m, xc, rows, x_dtype, static_cast<double *>(proba), m->opt_check_finite ? flag : nullptr, st);
                     });
+}
+
+int tcsdn_kmeans_transform(tcsdn_model_t *m, const void *x, int64_t n, int32_t d, int32_t x_dtype, int32_t x_loc,
+                           double *dist_out, void *cuda_stream) {
+    if (!m) { set_error("model is NULL"); return TCSDN_EINVAL; }
+    if (m->kind != TCSDN_KIND_KMEANS) { set_error("transform needs a KMeans handle"); return TCSDN_EINVAL; }
+    TCSDN_TRY(check_call(m, x, n, d, x_dtype, x_loc, dist_out, "dist_out"));
+    if (n == 0) return TCSDN_OK;
+    DeviceGuard guard;
+    TCSDN_TRY(begin_call(m, guard));
+    if (x_loc == TCSDN_DEVICE)   // sticky non-finite flag, read by tcsdn_sync_check (as for tcsdn_predict)
+        return launch_kmeans_surface(m, x, n, x_dtype, false, dist_out, m->opt_check_finite ? m->d_flag : nullptr,
+                                     static_cast<cudaStream_t>(cuda_stream));
+    // ~16 MiB of rows and distances per chunk, like the other streaming scorers; the distances (8 k bytes a row) are
+    // written straight into the caller's array, as kneighbors does
+    const size_t row_bytes = (size_t)d * (x_dtype == TCSDN_F32 ? 4 : 8);
+    void *const out[2] = {dist_out, nullptr};
+    const size_t out_row[2] = {(size_t)m->n_classes * sizeof(double), 0};
+    return run_host(m, x, n, row_bytes, chunk_rows(16u << 20, row_bytes + out_row[0]), out, out_row, false,
+                    [&](const void *xc, int64_t rows, void *dist, void *, int32_t *flag, cudaStream_t st) {
+                        return launch_kmeans_surface(m, xc, rows, x_dtype, false, static_cast<double *>(dist),
+                                                     m->opt_check_finite ? flag : nullptr, st);
+                    });
+}
+
+int tcsdn_kmeans_score(tcsdn_model_t *m, const void *x, int64_t n, int32_t d, int32_t x_dtype, int32_t x_loc,
+                       double *inertia_out, void *cuda_stream) {
+    if (!m) { set_error("model is NULL"); return TCSDN_EINVAL; }
+    if (m->kind != TCSDN_KIND_KMEANS) { set_error("score needs a KMeans handle"); return TCSDN_EINVAL; }
+    if (!inertia_out) { set_error("inertia_out is NULL"); return TCSDN_EINVAL; }
+    TCSDN_TRY(check_call(m, x, n, d, x_dtype, x_loc, inertia_out, "inertia_out"));
+    *inertia_out = 0.0;
+    if (n == 0) return TCSDN_OK;
+    DeviceGuard guard;
+    TCSDN_TRY(begin_call(m, guard));
+    // Every launch writes its CTAs' partial sums into its own slice of `part` (zeros where it has fewer CTAs than slots); one
+    // ordered sum over all slices gives the total, so a call on the same rows returns the same bits.
+    const size_t row_bytes = (size_t)d * (x_dtype == TCSDN_F32 ? 4 : 8);
+    const int64_t grid_cap = (int64_t)m->sm_count * 8;
+    int64_t chunk = n, slices = 1, slice = grid_cap;
+    if (x_loc == TCSDN_HOST) {
+        chunk = m->opt_chunk_rows > 0 ? m->opt_chunk_rows : chunk_rows(16u << 20, row_bytes);   // run_host's chunks
+        if (chunk > n) chunk = n;
+        slices = (n + chunk - 1) / chunk;
+        slice = std::min<int64_t>(grid_cap, (chunk + 255) / 256);   // no kernel runs more CTAs than 256-row tiles / blocks
+    }
+    const int64_t cells = slices * slice + 1;
+    double *part = nullptr;
+    TCSDN_CUDA(cudaMalloc((void **)&part, (size_t)cells * sizeof(double)));
+    struct Free { double *p; ~Free() { cudaFree(p); } } free_part{part};
+    double *total = part + slices * slice;
+    if (x_loc == TCSDN_DEVICE) {   // sticky non-finite flag, read by tcsdn_sync_check (as for tcsdn_predict)
+        cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+        TCSDN_CUDA(cudaMemsetAsync(part, 0, (size_t)cells * sizeof(double), st));
+        TCSDN_TRY(launch_kmeans_surface(m, x, n, x_dtype, true, part, m->opt_check_finite ? m->d_flag : nullptr, st));
+        TCSDN_TRY(launch_ordered_sum(part, slices * slice, total, st));
+        TCSDN_CUDA(cudaMemcpyAsync(inertia_out, total, sizeof(double), cudaMemcpyDeviceToHost, st));
+        TCSDN_CUDA(cudaStreamSynchronize(st));
+        return TCSDN_OK;
+    }
+    // the pipeline's streams do not wait for the legacy stream: the zeros are in place before it starts
+    TCSDN_CUDA(cudaMemset(part, 0, (size_t)cells * sizeof(double)));
+    TCSDN_CUDA(cudaStreamSynchronize(nullptr));
+    int64_t next = 0;
+    void *const out[2] = {nullptr, nullptr};
+    const size_t out_row[2] = {0, 0};
+    TCSDN_TRY(run_host(m, x, n, row_bytes, chunk, out, out_row, false,
+                       [&](const void *xc, int64_t rows, void *, void *, int32_t *flag, cudaStream_t st) {
+                           return launch_kmeans_surface(m, xc, rows, x_dtype, true, part + (next++) * slice,
+                                                        m->opt_check_finite ? flag : nullptr, st);
+                       }));
+    TCSDN_TRY(launch_ordered_sum(part, slices * slice, total, nullptr));
+    TCSDN_CUDA(cudaMemcpy(inertia_out, total, sizeof(double), cudaMemcpyDeviceToHost));
+    return TCSDN_OK;
 }
 
 int tcsdn_knn_kneighbors(tcsdn_model_t *m, const void *x, int64_t n, int32_t d, int32_t x_dtype, int32_t x_loc,

@@ -38,7 +38,8 @@ constexpr int kMaxClasses = 64;
 // Parameters of the streaming scorers, passed by value (__grid_constant__) so that fully unrolled
 // kernels read them as constant-bank operands.  a/b are [rows][d] (row stride d), c is [rows].
 //   linear : s_r = c_r + sum_j a_rj x_j                         (a = coef, c = intercept), argmax
-//   kmeans : s_r = c_r + sum_j a_rj x_j                         (a = -2 centers, c = ||c||^2), argmin
+//   kmeans : s_r = c_r + sum_j a_rj x_j                         (a = -2 centers, c = ||c||^2), argmin; b = centers
+//            (KMeans.transform and KMeans.score, scorers.cu)
 //   gnb    : s_r = c_r - sum_j (a_rj x_j - b_rj)^2              (a = 1/sqrt(2 var), b = theta * a), argmax
 struct ScorerParams {
     double a[kMaxClassesFast * 16];
@@ -209,6 +210,12 @@ int check_x(const tcsdn_model *m, int32_t d, int32_t x_dtype);
 // `flag` (nullable): device int32 the kernels OR 1 into when a row holds NaN/inf.
 int launch_scorer(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, double *scores,
                   int32_t *flag, cudaStream_t st, const GatherOut *gather = nullptr);
+// KMeans.transform (inertia false: dist [n][k], sqrt of kmeans_dist.cuh's squared distance) and KMeans.score (inertia true:
+// one partial sum per CTA into out[0 .. m->sm_count * 8), the largest grid; slots a launch does not use are left alone)
+int launch_kmeans_surface(tcsdn_model *m, const void *x, int64_t n, int dtype, bool inertia, double *out, int32_t *flag,
+                          cudaStream_t st);
+// *out = v[0] + ... + v[count - 1] in a fixed order (device pointers)
+int launch_ordered_sum(const double *v, int64_t count, double *out, cudaStream_t st);
 int launch_forest(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *labels, double *scores,
                   int32_t *flag, cudaStream_t st);
 int launch_knn_exact(tcsdn_model *m, const void *x, int64_t n, int dtype, const KnnCall &call, int32_t *flag, cudaStream_t st);

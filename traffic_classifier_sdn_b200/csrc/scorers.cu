@@ -26,12 +26,33 @@
 #include <utility>
 
 #include "common.h"
+#include "kmeans_dist.cuh"
 
 namespace tcsdn {
 
 constexpr int kStages = 3;     // shared-memory ring depth; tile = kThreads x kRPT rows (template parameters below)
 
-enum : int { KIND_AFFINE_MAX = 0, KIND_AFFINE_MIN = 1, KIND_GNB = 2 };
+// KMeans handles also take the two kinds of KMeans.transform and KMeans.score (launch_kmeans_surface).  Their centres are
+// P.b / d_b (tcsdn_kmeans_create):
+//   KIND_KM_DIST     scores[row][r] = sqrt(km_sqdist(x, c_r)), correctly rounded; no labels
+//   KIND_KM_INERTIA  predict's label (the KIND_AFFINE_MIN argmin), then km_sqdist(x, c_label) summed per thread in row order,
+//                    per CTA in a fixed order: scores[blockIdx.x] is the CTA's partial sum; no labels
+enum : int { KIND_AFFINE_MAX = 0, KIND_AFFINE_MIN = 1, KIND_GNB = 2, KIND_KM_DIST = 3, KIND_KM_INERTIA = 4 };
+
+// Sum of one value per thread, in a fixed order (a shuffle tree per warp, then the warps in order); the result is valid
+// in thread 0.  Every thread of the block must call it.
+template <int kThreads>
+__device__ __forceinline__ double block_sum_fixed(double v) {
+    __shared__ double warp_sums[kThreads / 32];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = __dadd_rn(v, __shfl_down_sync(0xffffffffu, v, o));
+    if ((threadIdx.x & 31) == 0) warp_sums[threadIdx.x >> 5] = v;
+    __syncthreads();
+    double s = 0.0;
+    if (threadIdx.x == 0)
+        for (int w = 0; w < kThreads / 32; ++w) s = __dadd_rn(s, warp_sums[w]);
+    return s;
+}
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) {
     return static_cast<uint32_t>(__cvta_generic_to_shared(p));
@@ -283,6 +304,7 @@ __global__ void __launch_bounds__(kThreads) scorer_tiled_kernel(const __grid_con
     }
 
     float nf = 0.f;
+    double inertia = 0.0;   // KIND_KM_INERTIA: this thread's rows, in the order it scores them
     // Every thread has lifted its rows out of the stage: refill it with the tile kStages rounds ahead.  The bulk copy (async
     // proxy) must not overtake shared loads that are still in flight, and neither BAR.SYNC nor a MEMBAR.CTA in front of it
     // waits for those (see engine_core.cuh for the hazard): the fp32 pre-pass, whose loaded values are consumed only after the
@@ -350,6 +372,28 @@ __global__ void __launch_bounds__(kThreads) scorer_tiled_kernel(const __grid_con
             }
         }
         release(tile, stage);
+        if constexpr (KIND == KIND_KM_DIST || KIND == KIND_KM_INERTIA) {
+            int arg[kRPT];
+            if constexpr (KIND == KIND_KM_INERTIA) {
+                double s[kRPT][R];
+                score_rows<D, R, KIND_AFFINE_MIN, kRPT>(P, x, s, arg);
+            }
+#pragma unroll
+            for (int q = 0; q < kRPT; ++q) {
+                const int64_t row = row0 + q * kThreads + tid;
+                if (row >= n) continue;
+                const auto xq = [&](int j) { return x[q][j]; };
+                if constexpr (KIND == KIND_KM_DIST) {
+#pragma unroll
+                    for (int r = 0; r < R; ++r)
+                        scores[row * R + r] = __dsqrt_rn(km_sqdist(D, xq, [&](int j) { return P.b[r * D + j]; }));
+                } else {
+                    const int c = arg[q];
+                    inertia = __dadd_rn(inertia, km_sqdist(D, xq, [&](int j) { return P.b[c * D + j]; }));
+                }
+            }
+            continue;
+        }
         double s[kRPT][R];
         int arg[kRPT];
         score_rows<D, R, KIND, kRPT>(P, x, s, arg);
@@ -362,6 +406,10 @@ __global__ void __launch_bounds__(kThreads) scorer_tiled_kernel(const __grid_con
             }
         }
         store_labels(row0, arg);
+    }
+    if constexpr (KIND == KIND_KM_INERTIA) {
+        const double cta = block_sum_fixed<kThreads>(inertia);
+        if (tid == 0) scores[blockIdx.x] = cta;
     }
     if (flag && nf != nf) atomicOr(flag, 1);
 }
@@ -401,11 +449,49 @@ __global__ void __launch_bounds__(256) scorer_generic_kernel(const T *__restrict
     if (flag && nf != nf) atomicOr(flag, 1);
 }
 
+// Generic path of KIND_KM_DIST / KIND_KM_INERTIA (any d, any k, unaligned X): the arithmetic of the tiled kinds, with the
+// parameters from HBM.  KIND_KM_INERTIA writes one partial sum per block to out[blockIdx.x].
+template <typename T, int KIND>
+__global__ void __launch_bounds__(256) kmeans_generic_kernel(const T *__restrict__ X, int64_t n, int d, int R,
+                                                             const double *__restrict__ A, const double *__restrict__ Cc,
+                                                             const double *__restrict__ Ctr, double *__restrict__ out,
+                                                             int32_t *flag) {
+    float nf = 0.f;
+    double inertia = 0.0;
+    for (int64_t row = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; row < n; row += (int64_t)gridDim.x * blockDim.x) {
+        const T *x = X + row * d;
+        const auto xr = [&](int j) { return static_cast<double>(x[j]); };
+        if constexpr (KIND == KIND_KM_DIST) {
+            for (int r = 0; r < R; ++r) {
+                const double *c = Ctr + (int64_t)r * d;
+                out[row * R + r] = __dsqrt_rn(km_sqdist(d, xr, [&](int j) { return c[j]; }));
+            }
+        } else {
+            int arg = 0;
+            double best = 0.0;
+            for (int r = 0; r < R; ++r) {   // scorer_generic_kernel's KIND_AFFINE_MIN label
+                double acc = Cc[r];
+                for (int j = 0; j < d; ++j) acc = fma(static_cast<double>(x[j]), A[(int64_t)r * d + j], acc);
+                if (r == 0 || acc < best) { best = acc; arg = r; }
+            }
+            const double *c = Ctr + (int64_t)arg * d;
+            inertia = __dadd_rn(inertia, km_sqdist(d, xr, [&](int j) { return c[j]; }));
+        }
+        for (int j = 0; j < d; ++j) nf += static_cast<float>(x[j] * static_cast<T>(0));
+    }
+    if constexpr (KIND == KIND_KM_INERTIA) {
+        const double cta = block_sum_fixed<256>(inertia);
+        if (threadIdx.x == 0) out[blockIdx.x] = cta;
+    }
+    if (flag && nf != nf) atomicOr(flag, 1);
+}
+
 template <typename T, int D, int R, int KIND, int kThreads, int kRPT>
 static int launch_tiled_cfg(tcsdn_model *m, const T *x, int64_t n, int32_t *labels, double *scores, int32_t *flag,
                             cudaStream_t st, int ctas_per_sm, const GatherOut &G) {
     constexpr int kTile = kThreads * kRPT;
-    constexpr bool kCanGather = sizeof(T) == 4;   // the fused gather is instantiated for float32 rows (comm.cu checks)
+    // the fused gather is instantiated for float32 rows (comm.cu checks) of the label kinds
+    constexpr bool kCanGather = sizeof(T) == 4 && KIND <= KIND_GNB;
     if (G.world && !kCanGather) { set_error("fused gather: float32 rows only"); return TCSDN_EINVAL; }
     auto kern = (kCanGather && G.world) ? scorer_tiled_kernel<T, D, R, KIND, kThreads, kRPT, kCanGather>
                                         : scorer_tiled_kernel<T, D, R, KIND, kThreads, kRPT, false>;
@@ -501,6 +587,8 @@ template <typename T, int D>
 static int dispatch_kind(tcsdn_model *m, int kind, const T *x, int64_t n, int32_t *labels, double *scores,
                          int32_t *flag, cudaStream_t st, const GatherOut &G) {
     if (kind == KIND_GNB) return dispatch_rows<T, D, KIND_GNB>(m, x, n, labels, scores, flag, st, G);
+    if (kind == KIND_KM_DIST) return dispatch_rows<T, D, KIND_KM_DIST>(m, x, n, labels, scores, flag, st, G);
+    if (kind == KIND_KM_INERTIA) return dispatch_rows<T, D, KIND_KM_INERTIA>(m, x, n, labels, scores, flag, st, G);
     if (kind == KIND_AFFINE_MIN) return dispatch_rows<T, D, KIND_AFFINE_MIN>(m, x, n, labels, scores, flag, st, G);
     return dispatch_rows<T, D, KIND_AFFINE_MAX>(m, x, n, labels, scores, flag, st, G);
 }
@@ -545,6 +633,12 @@ static int launch_scorer_t(tcsdn_model *m, int kind, const T *x, int64_t n, int3
     int64_t blocks = (n + 255) / 256;
     int64_t cap = (int64_t)m->sm_count * 8;
     if (blocks > cap) blocks = cap;
+    if (kind == KIND_KM_DIST || kind == KIND_KM_INERTIA) {
+        auto kern = kind == KIND_KM_DIST ? kmeans_generic_kernel<T, KIND_KM_DIST> : kmeans_generic_kernel<T, KIND_KM_INERTIA>;
+        kern<<<(unsigned)blocks, 256, 0, st>>>(x, n, m->d, m->n_classes, m->d_a, m->d_c, m->d_b, scores, flag);
+        TCSDN_CUDA(cudaGetLastError());
+        return TCSDN_OK;
+    }
     scorer_generic_kernel<T><<<(unsigned)blocks, 256, 0, st>>>(x, n, m->d, m->n_classes, kind, m->d_a, m->d_b,
                                                                m->d_c, labels, scores, flag);
     TCSDN_CUDA(cudaGetLastError());
@@ -561,6 +655,31 @@ int launch_scorer(tcsdn_model *m, const void *x, int64_t n, int dtype, int32_t *
     m->stats[0] += 1;
     if (dtype == TCSDN_F32) return launch_scorer_t<float>(m, kind, static_cast<const float *>(x), n, labels, scores, flag, st, G);
     return launch_scorer_t<double>(m, kind, static_cast<const double *>(x), n, labels, scores, flag, st, G);
+}
+
+// out[0] = the sum of v[0 .. count) in a fixed order (thread t adds v[t], v[t + 256], ... in turn, then block_sum_fixed)
+__global__ void __launch_bounds__(256) ordered_sum_kernel(const double *__restrict__ v, int64_t count, double *out) {
+    double s = 0.0;
+    for (int64_t i = threadIdx.x; i < count; i += 256) s = __dadd_rn(s, v[i]);
+    s = block_sum_fixed<256>(s);
+    if (threadIdx.x == 0) out[0] = s;
+}
+
+int launch_kmeans_surface(tcsdn_model *m, const void *x, int64_t n, int dtype, bool inertia, double *out, int32_t *flag,
+                          cudaStream_t st) {
+    if (n == 0) return TCSDN_OK;
+    GatherOut G;
+    memset(&G, 0, sizeof(G));
+    const int kind = inertia ? KIND_KM_INERTIA : KIND_KM_DIST;
+    m->stats[0] += 1;
+    if (dtype == TCSDN_F32) return launch_scorer_t<float>(m, kind, static_cast<const float *>(x), n, nullptr, out, flag, st, G);
+    return launch_scorer_t<double>(m, kind, static_cast<const double *>(x), n, nullptr, out, flag, st, G);
+}
+
+int launch_ordered_sum(const double *v, int64_t count, double *out, cudaStream_t st) {
+    ordered_sum_kernel<<<1, 256, 0, st>>>(v, count, out);
+    TCSDN_CUDA(cudaGetLastError());
+    return TCSDN_OK;
 }
 
 #endif   // TCSDN_SCORER_D

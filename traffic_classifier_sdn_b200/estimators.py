@@ -8,7 +8,7 @@ These classes are the drop-in for the objects the reference gets from ``pickle.l
   KMeans); ``classes_``, ``n_features_in_``; ``decision_function`` (LogisticRegression, SVC),
   ``predict_proba`` (GaussianNB, KNeighborsClassifier, RandomForestClassifier, SVC(probability=True)), ``predict_log_proba`` /
   ``transform`` where sklearn has them and they are a closed form of the kernel's score matrix;
-  ``kneighbors`` (KNeighborsClassifier);
+  ``kneighbors`` (KNeighborsClassifier); ``transform``, ``fit_transform`` and ``score`` (KMeans, their own kernels);
 * ``ValueError`` on a wrong feature count or NaN/inf input, ``NotFittedError`` before ``fit``;
   inputs are never modified, outputs are freshly allocated.
 
@@ -36,7 +36,7 @@ except Exception:  # pragma: no cover - sklearn absent
         pass
 
 __all__ = ["LogisticRegression", "GaussianNB", "KMeans", "KNeighborsClassifier", "SVC",
-           "RandomForestClassifier", "from_spec", "from_sklearn", "load_model", "NotFittedError"]
+           "RandomForestClassifier", "from_spec", "from_sklearn", "load_model", "kmeans_plusplus", "NotFittedError"]
 
 
 def _is_torch_cuda(x) -> bool:
@@ -390,9 +390,10 @@ class KMeans(_Base):
         return idx.astype(np.int32, copy=False)
 
     def _fit_gpu(self, X, y, strict):
-        """Lloyd iterations on the GPU (tcsdn_kmeans_fit) from ONE set of initial centres: an ``init`` array, or
-        scikit-learn's k-means++ seeding run on the host with this estimator's ``random_state`` (the same centres
-        ``sklearn.cluster.KMeans(n_init=1)`` starts from).  Several restarts (n_init > 1) stay with scikit-learn."""
+        """Lloyd iterations on the GPU (tcsdn_kmeans_fit) from ONE set of initial centres: an ``init`` array, or k-means++
+        seeding on the GPU (kmeans_plusplus) with scikit-learn's draws from this estimator's ``random_state``.  scikit-learn
+        seeds on the mean-centred rows, this seeding on the rows as given: the centres are the same unless a draw falls
+        within rounding of a prefix-sum boundary.  Several restarts (n_init > 1) stay with scikit-learn."""
         p = self._params
         k = int(p.get("n_clusters", 8))
         init = p.get("init", "k-means++")
@@ -414,14 +415,8 @@ class KMeans(_Base):
             if c0.shape != (k, d):
                 raise ValueError(f"The shape of the initial centers {c0.shape} does not match the number of clusters {k} "
                                  f"and features {d}.")
-        else:
-            from sklearn.cluster import kmeans_plusplus
-            from sklearn.utils import check_random_state
-            host = keep.cpu().numpy() if loc == _lib.DEVICE else keep
-            host = np.asarray(host, np.float64)
-            mean = host.mean(axis=0)                      # sklearn seeds on the mean-centred rows
-            c0, _ = kmeans_plusplus(host - mean, k, random_state=check_random_state(p.get("random_state")))
-            c0 = np.ascontiguousarray(c0 + mean, np.float64)
+        else:   # the rows stay where they are: host rows are uploaded once more by the fit below
+            c0 = _seed_plusplus(ptr, n, d, dt, loc, k, p.get("random_state"), None)[0]
         ctr = np.empty((k, d))
         inertia, n_iter = C.c_double(0.0), C.c_int32(0)
         if loc == _lib.HOST:
@@ -441,6 +436,88 @@ class KMeans(_Base):
 
     def fit_predict(self, X, y=None):
         return self.fit(X).predict(X)
+
+    def fit_transform(self, X, y=None):
+        """``fit(X)`` followed by ``transform(X)``."""
+        return self.fit(X).transform(X)
+
+    def transform(self, X):
+        """sk:cluster/_kmeans.py ``transform``: the distance of every row to every centre, [n, n_clusters] float64
+        (tcsdn_kmeans_transform: scikit-learn's _euclidean_dense_dense in fp64, correctly rounded sqrt).  A CUDA
+        ``torch.Tensor`` gives a CUDA tensor, enqueued on the current stream (``sync_check()`` reports NaN/inf rows)."""
+        self._check_fitted()
+        X, n, d, dt, loc = _rows(X)
+        if d != self.n_features_in_:
+            raise ValueError(f"X has {d} features, but {type(self).__name__} is expecting {self.n_features_in_} features as input")
+        lib = _lib.load()
+        return _call(X, loc, [((n, len(self.cluster_centers_)), np.float64)],
+                     lambda x, o, st: lib.tcsdn_kmeans_transform(self._handle, x, n, d, dt, loc, o[0], st))[0]
+
+    def score(self, X, y=None, sample_weight=None):
+        """sk:cluster/_kmeans.py ``score``: minus the inertia of X against the fitted centres, each row with the centre
+        ``predict`` gives it (tcsdn_kmeans_score).  Unit weights only."""
+        if sample_weight is not None:
+            raise ValueError("KMeans.score supports sample_weight=None only")
+        self._check_fitted()
+        X, n, d, dt, loc = _rows(X)
+        if d != self.n_features_in_:
+            raise ValueError(f"X has {d} features, but {type(self).__name__} is expecting {self.n_features_in_} features as input")
+        lib = _lib.load()
+        inertia = C.c_double(0.0)
+        if loc == _lib.DEVICE:
+            import torch
+            with torch.cuda.device(X.device):
+                _lib.check(lib.tcsdn_kmeans_score(self._handle, X.data_ptr(), n, d, dt, loc, C.byref(inertia),
+                                                  torch.cuda.current_stream().cuda_stream))
+            self.sync_check()
+        else:
+            _lib.check(lib.tcsdn_kmeans_score(self._handle, _lib.ptr(X), n, d, dt, loc, C.byref(inertia), None))
+        return -float(inertia.value)
+
+
+def _seed_plusplus(ptr, n, d, dt, loc, k, random_state, n_local_trials):
+    """tcsdn_kmeans_plusplus on rows from _Base._fit_rows, with scikit-learn's draws: -> (centers [k, d] float64, indices)."""
+    from sklearn.utils import check_random_state
+    if k > n:
+        raise ValueError(f"n_samples={n} should be >= n_clusters={k}.")
+    if n_local_trials is None:
+        n_local_trials = 2 + int(np.log(k))
+    elif int(n_local_trials) < 1:
+        raise ValueError(f"n_local_trials must be >= 1, got {n_local_trials}")
+    L = int(n_local_trials)
+    # sk:cluster/_kmeans.py:_kmeans_plusplus with sample_weight = ones: the draws do not depend on the data, so all of them
+    # are made here, in scikit-learn's order
+    rs = check_random_state(random_state)
+    w = np.ones(n)
+    first = int(rs.choice(n, p=w / w.sum()))
+    u = np.ascontiguousarray(np.concatenate([rs.uniform(size=L) for _ in range(k - 1)]) if k > 1 else np.zeros(1))
+    centers = np.empty((k, d))
+    indices = np.empty(k, np.int64)
+    st = None
+    if loc == _lib.DEVICE:
+        import torch
+        st = torch.cuda.current_stream().cuda_stream
+    _lib.check(_lib.load().tcsdn_kmeans_plusplus(ptr, n, d, k, dt, loc, first, L, _p(u, _lib._f64p), _p(indices, _lib._i64p),
+                                                 _p(centers, _lib._f64p), st))
+    return centers, indices
+
+
+def kmeans_plusplus(X, n_clusters, *, random_state=None, n_local_trials=None):
+    """sklearn.cluster.kmeans_plusplus on the GPU (tcsdn_kmeans_plusplus), unit sample weights: ``(centers, indices)``,
+    centers [n_clusters, n_features] in X's dtype, indices int64.  The random numbers are scikit-learn's, drawn in its order
+    from ``check_random_state(random_state)``; the distances and sums are fp64 on the GPU.  X may be a CUDA
+    ``torch.Tensor`` (its rows are not copied to the host); the results are numpy arrays either way."""
+    n_clusters = int(n_clusters)
+    if n_clusters < 1:
+        raise ValueError(f"n_clusters must be >= 1, got {n_clusters}")
+    ptr, n, d, dt, loc, keep = _Base._fit_rows(X)
+    if loc == _lib.DEVICE:
+        import torch
+        with torch.cuda.device(keep.device):
+            centers, indices = _seed_plusplus(ptr, n, d, dt, loc, n_clusters, random_state, n_local_trials)
+    else:
+        centers, indices = _seed_plusplus(ptr, n, d, dt, loc, n_clusters, random_state, n_local_trials)
+    return centers.astype(np.float32 if dt == _lib.F32 else np.float64, copy=False), indices
 
 
 class KNeighborsClassifier(_Base):
