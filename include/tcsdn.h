@@ -259,7 +259,7 @@ int tcsdn_svc_ovr_from_ovo(const double *dec, int64_t n, int32_t n_classes, int3
                            void *cuda_stream);
 
 /* ---- N3 (next row): `.fit` of the two cheap models on the GPU -------------------------------------
- * (the other four estimators keep importing fitted parameters from scikit-learn).  X [n][d] float32/float64 and
+ * (RandomForestClassifier has tcsdn_forest_fit below; the other three keep importing fitted parameters from scikit-learn).  X [n][d] float32/float64 and
  * y / labels_out live where `loc` says; the small outputs (theta, var, ..., centers_out) are HOST arrays.
  * Sums are fp64 and deterministic but not in numpy's order: results agree with scikit-learn to ~1e-13 relative.
  * float32 rows are fitted in fp64 (scikit-learn's fit of the widened rows).  d <= 255.
@@ -297,6 +297,37 @@ int tcsdn_kmeans_fit(const void *x, int64_t n, int32_t d, int32_t k, int32_t x_d
 int tcsdn_kmeans_plusplus(const void *x, int64_t n, int32_t d, int32_t k, int32_t x_dtype, int32_t loc, int64_t first_index,
                           int32_t n_local_trials, const double *uniforms, int64_t *indices_out, double *centers_out,
                           void *cuda_stream);
+
+/* tcsdn_forest_fit  RandomForestClassifier(criterion='gini').fit (sk:ensemble/_forest.py, sk:tree/_tree.pyx
+ *                   DepthFirstTreeBuilder, sk:tree/_splitter.pyx node_split_best, sk:tree/_criterion.pyx Gini): the trees
+ *                   scikit-learn 1.9 grows, node for node and bit for bit, given its random numbers.  The caller draws them
+ *                   in scikit-learn's order (traffic_classifier_sdn_b200.estimators.forest_fit_plan): per tree t,
+ *                   bootstrap_idx [n_trees][n_boot] (HOST int32; NULL: bootstrap=False, every row weight 1) and
+ *                   rand_r_seeds [n_trees] (HOST, the splitter's rand_r_state).  X [n][d] float32/float64 and y [n] class
+ *                   index in [0, n_classes) live where `loc` says; X is rounded to float32 (to nearest) as scikit-learn
+ *                   does; device rows are never copied to the host.  Parameters are the resolved ones of
+ *                   BaseDecisionTree._fit (max_depth, min_samples_split already max(., 2 min_samples_leaf), max_features
+ *                   in [1, d]).  node_capacity: nodes per tree of the first attempt (0: min(2 m - 1, 16384) with m = n, or
+ *                   min(n, n_boot) with bootstrap); a tree that outgrows it is grown again, deterministically, with room
+ *                   for 2 m - 1 nodes, which any tree fits.
+ *                   d <= 255, n_classes <= 32, n and n_boot < 2^31; TCSDN_EINVAL otherwise or for a class index out of
+ *                   range, before any tree is grown; TCSDN_ENONFINITE for NaN / inf rows (after the cast to float32);
+ *                   TCSDN_ECUDA with a message when device memory runs out.  The call returns when the trees are on
+ *                   the host, in *out.
+ * tcsdn_forest_fit_nodes  tree_offsets [n_trees + 1] (HOST): tree t owns nodes [tree_offsets[t], tree_offsets[t+1]).
+ * tcsdn_forest_fit_read   the per-tree `tree_` arrays concatenated, node indices local to each tree, in
+ *                   tcsdn_forest_create's layout: children_left / children_right (-1: leaf), feature and threshold (-2 on
+ *                   leaves), value [N][n_classes] (class fractions), impurity, n_node_samples, weighted_n_node_samples
+ *                   (HOST arrays, N = tree_offsets[n_trees]). */
+typedef struct tcsdn_forest_fit tcsdn_forest_fit_t;
+int tcsdn_forest_fit(const void *x, const int32_t *y, int64_t n, int32_t d, int32_t n_classes, int32_t x_dtype, int32_t loc,
+                     int32_t n_trees, const int32_t *bootstrap_idx, int64_t n_boot, const uint32_t *rand_r_seeds,
+                     int32_t max_features, int32_t max_depth, int64_t min_samples_split, int64_t min_samples_leaf,
+                     double min_impurity_decrease, int64_t node_capacity, tcsdn_forest_fit_t **out, void *cuda_stream);
+int tcsdn_forest_fit_nodes(const tcsdn_forest_fit_t *f, int64_t *tree_offsets);
+int tcsdn_forest_fit_read(const tcsdn_forest_fit_t *f, int32_t *left, int32_t *right, int32_t *feature, double *threshold,
+                          double *value, double *impurity, int64_t *n_node_samples, double *weighted_n_node_samples);
+void tcsdn_forest_fit_free(tcsdn_forest_fit_t *f);
 
 /* ---- multi-GPU (SURVEY 8e): one process per GPU, rows sharded, models replicated ------------------
  * predict() never communicates: rank r classifies its contiguous block of n_block = ceil(n / world) rows.  The only

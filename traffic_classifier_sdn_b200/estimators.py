@@ -98,7 +98,8 @@ class _Base:
 
     def fit(self, X, y=None, backend="auto"):
         """Train, then move the fitted parameters to HBM.  GaussianNB and KMeans fit on the GPU (SURVEY row N3,
-        csrc/fit.cu) unless ``backend="sklearn"``; the other four train with scikit-learn on the host."""
+        csrc/fit.cu) unless ``backend="sklearn"``; RandomForestClassifier fits on the GPU with ``backend="gpu"``
+        (csrc/forest_fit.cu) and with scikit-learn on the host otherwise; the other three train with scikit-learn."""
         if backend not in ("auto", "gpu", "sklearn"):
             raise ValueError("backend must be 'auto', 'gpu' or 'sklearn'")
         if backend != "sklearn" and self._fit_gpu(X, y, strict=backend == "gpu"):
@@ -106,7 +107,7 @@ class _Base:
         est = self._sk_estimator()
         est.fit(X) if y is None and self._kind == "kmeans" else est.fit(X, y)
         self._adopt(modelio.spec_from_estimator(est))
-        for attr in ("n_iter_", "inertia_", "labels_", "feature_names_in_"):
+        for attr in ("n_iter_", "inertia_", "labels_", "feature_names_in_", "feature_importances_"):
             if hasattr(est, attr):
                 setattr(self, attr, getattr(est, attr))
         return self
@@ -743,6 +744,185 @@ class SVC(_Base):
         return super().predict(X)
 
 
+_FOREST_GPU_PARAMS = ("n_estimators", "criterion", "max_depth", "min_samples_split", "min_samples_leaf", "max_features",
+                      "bootstrap", "max_samples", "min_impurity_decrease", "random_state", "n_jobs", "verbose",
+                      "min_weight_fraction_leaf", "max_leaf_nodes", "class_weight", "monotonic_cst", "oob_score",
+                      "warm_start", "ccp_alpha")
+# parameters the GPU fit refuses unless they hold scikit-learn's default
+_FOREST_GPU_DEFAULTS = {"criterion": "gini", "min_weight_fraction_leaf": 0.0, "max_leaf_nodes": None, "class_weight": None,
+                        "monotonic_cst": None, "oob_score": False, "warm_start": False, "ccp_alpha": 0.0}
+
+
+def forest_fit_plan(params, n, d):
+    """Host half of RandomForestClassifier.fit (sk:ensemble/_forest.py fit, sk:tree/_classes.py BaseDecisionTree._fit) for
+    the GPU fit: the resolved tree parameters and every random number, drawn in scikit-learn's order.  -> dict with
+    ``n_trees``, ``max_depth``, ``min_samples_split``, ``min_samples_leaf``, ``max_features``, ``min_impurity_decrease``,
+    ``n_boot`` (0 without bootstrap), ``bootstrap_idx`` ([n_trees][n_boot] int32 or None) and ``rand_r_seeds``
+    ([n_trees] uint32, each tree splitter's ``rand_r_state``).  Raises ValueError naming a parameter it does not support."""
+    import numbers
+    from math import ceil
+    from sklearn.utils import check_random_state
+    p = dict(params)
+    for k in p:
+        if k not in _FOREST_GPU_PARAMS:
+            raise ValueError(f"RandomForestClassifier GPU fit: unknown parameter {k}")
+    for k, default in _FOREST_GPU_DEFAULTS.items():
+        v = p.get(k, default)
+        same = v is None if default is None else (type(v) is type(default) or isinstance(v, numbers.Real) and
+                                                  not isinstance(v, bool) and isinstance(default, float)) and v == default
+        if not same:
+            raise ValueError(f"RandomForestClassifier GPU fit: {k}={v!r} is not supported (only {k}={default!r})")
+    T = p.get("n_estimators", 100)
+    if not isinstance(T, numbers.Integral) or T < 1:
+        raise ValueError(f"n_estimators must be an integer >= 1, got {T!r}")
+    md = p.get("max_depth")
+    if md is not None and (not isinstance(md, numbers.Integral) or md < 1):
+        raise ValueError(f"max_depth must be None or an integer >= 1, got {md!r}")
+    max_depth = np.iinfo(np.int32).max if md is None else int(md)
+    msl, mss = p.get("min_samples_leaf", 1), p.get("min_samples_split", 2)
+    if isinstance(msl, numbers.Integral) and not isinstance(msl, bool) and msl >= 1:
+        msl = int(msl)
+    elif isinstance(msl, numbers.Real) and not isinstance(msl, numbers.Integral) and 0.0 < msl < 1.0:
+        msl = ceil(msl * n)
+    else:
+        raise ValueError(f"min_samples_leaf must be an integer >= 1 or a float in (0, 1), got {msl!r}")
+    if isinstance(mss, numbers.Integral) and not isinstance(mss, bool) and mss >= 2:
+        mss = int(mss)
+    elif isinstance(mss, numbers.Real) and not isinstance(mss, numbers.Integral) and 0.0 < mss <= 1.0:
+        mss = max(2, ceil(mss * n))
+    else:
+        raise ValueError(f"min_samples_split must be an integer >= 2 or a float in (0, 1], got {mss!r}")
+    mss = max(mss, 2 * msl)
+    mf = p.get("max_features", "sqrt")
+    if isinstance(mf, str) and mf in ("sqrt", "log2"):
+        mf = max(1, int(np.sqrt(d) if mf == "sqrt" else np.log2(d)))
+    elif mf is None:
+        mf = d
+    elif isinstance(mf, numbers.Integral) and not isinstance(mf, bool) and 1 <= mf <= d:
+        mf = int(mf)
+    elif isinstance(mf, numbers.Real) and not isinstance(mf, numbers.Integral) and 0.0 < mf <= 1.0:
+        mf = max(1, int(mf * d))
+    else:
+        raise ValueError(f"max_features must be 'sqrt', 'log2', None, an integer in [1, {d}] or a float in (0, 1], "
+                         f"got {mf!r}")
+    mid = p.get("min_impurity_decrease", 0.0)
+    if not isinstance(mid, numbers.Real) or isinstance(mid, bool) or not mid >= 0.0:
+        raise ValueError(f"min_impurity_decrease must be a float >= 0, got {mid!r}")
+    bootstrap, ms = p.get("bootstrap", True), p.get("max_samples")
+    if not bootstrap and ms is not None:
+        raise ValueError("max_samples cannot be set if bootstrap=False")
+    n_boot = 0
+    if bootstrap:   # sk:ensemble/_bootstrap.py _get_n_samples_bootstrap
+        if ms is None:
+            n_boot = n
+        elif isinstance(ms, numbers.Integral) and not isinstance(ms, bool) and ms >= 1:
+            n_boot = int(ms)
+        elif isinstance(ms, numbers.Real) and not isinstance(ms, numbers.Integral) and 0.0 < ms <= 1.0:
+            n_boot = max(int(ms * n), 1)
+        else:
+            raise ValueError(f"max_samples must be None, an integer >= 1 or a float in (0, 1], got {ms!r}")
+    # sk:ensemble/_base.py _set_random_states: one seed per tree, in estimator order; then per tree a FRESH
+    # RandomState(seed) draws the bootstrap indices (_generate_sample_indices) and another the splitter's rand_r_state
+    # (sk:tree/_splitter.pyx Splitter.init)
+    rs = check_random_state(p.get("random_state"))
+    seeds = [rs.randint(np.iinfo(np.int32).max) for _ in range(T)]
+    idx = np.empty((T, n_boot), np.int32) if bootstrap else None
+    rr = np.empty(T, np.uint32)
+    for t, s in enumerate(seeds):
+        if bootstrap:
+            idx[t] = np.random.RandomState(s).randint(0, n, n_boot)
+        rr[t] = np.random.RandomState(s).randint(0, 2147483647)
+    return dict(n_trees=int(T), max_depth=int(max_depth), min_samples_split=int(mss), min_samples_leaf=int(msl),
+                max_features=int(mf), min_impurity_decrease=float(mid), n_boot=int(n_boot), bootstrap_idx=idx,
+                rand_r_seeds=rr)
+
+
+def forest_fit(X, y, params, node_capacity=0):
+    """RandomForestClassifier(**params).fit(X, y) on the GPU (tcsdn_forest_fit, criterion='gini', no sample or class
+    weights): -> (classes_, dict of the concatenated per-tree node arrays with ``tree_offsets`` and ``n_features``).  X:
+    numpy rows or a CUDA tensor (its rows are not copied to the host); y on the host or the device.  ``node_capacity``:
+    nodes per tree of the first attempt (0: the library's default)."""
+    if y is None:
+        raise ValueError("RandomForestClassifier.fit needs y")
+    ptr, n, d, dt, loc, keep = _Base._fit_rows(X)
+    if _is_torch_cuda(y):
+        y = y.cpu().numpy()
+    y = np.asarray(y)
+    if y.ndim != 1:
+        raise ValueError("the GPU fit supports a 1-D y (one output)")
+    if len(y) != n:
+        raise ValueError(f"Found input variables with inconsistent numbers of samples: [{n}, {len(y)}]")
+    classes, yi = np.unique(y, return_inverse=True)
+    if len(classes) > 32 or d > 255 or n >= 2 ** 31:
+        raise ValueError(f"the GPU fit supports at most 32 classes, 255 features and 2^31 - 1 rows "
+                         f"(got {len(classes)}, {d} and {n})")
+    plan = forest_fit_plan(params, n, d)
+    yi = np.ascontiguousarray(yi, np.int32)
+    ydev = None
+    if loc == _lib.DEVICE:
+        import torch
+        ydev = torch.from_numpy(yi).to(keep.device)
+        yptr = C.c_void_p(ydev.data_ptr())
+    else:
+        yptr = _p(yi, C.c_void_p)
+    boot = plan["bootstrap_idx"]
+    if boot is not None and plan["n_boot"] >= 2 ** 31:
+        raise ValueError(f"max_samples: the GPU fit draws fewer than 2^31 rows per tree (got {plan['n_boot']})")
+    T, Cn, lib = plan["n_trees"], len(classes), _lib.load()
+    h = C.c_void_p()
+    st = None
+    if loc == _lib.DEVICE:
+        import torch
+        st = torch.cuda.current_stream(keep.device).cuda_stream
+    _lib.check(lib.tcsdn_forest_fit(ptr, yptr, n, d, Cn, dt, loc, T, None if boot is None else _p(boot, C.c_void_p),
+                                    plan["n_boot"], _p(plan["rand_r_seeds"], C.c_void_p), plan["max_features"],
+                                    plan["max_depth"], plan["min_samples_split"], plan["min_samples_leaf"],
+                                    plan["min_impurity_decrease"], int(node_capacity), C.byref(h), st))
+    try:
+        offs = np.empty(T + 1, np.int64)
+        _lib.check(lib.tcsdn_forest_fit_nodes(h, _p(offs, _lib._i64p)))
+        N = int(offs[-1])
+        a = dict(left=np.empty(N, np.int32), right=np.empty(N, np.int32), feature=np.empty(N, np.int32),
+                 threshold=np.empty(N), value=np.empty((N, Cn)), impurity=np.empty(N),
+                 n_node_samples=np.empty(N, np.int64), weighted_n_node_samples=np.empty(N))
+        _lib.check(lib.tcsdn_forest_fit_read(h, _p(a["left"], _lib._i32p), _p(a["right"], _lib._i32p),
+                                             _p(a["feature"], _lib._i32p), _p(a["threshold"], _lib._f64p),
+                                             _p(a["value"], _lib._f64p), _p(a["impurity"], _lib._f64p),
+                                             _p(a["n_node_samples"], _lib._i64p),
+                                             _p(a["weighted_n_node_samples"], _lib._f64p)))
+    finally:
+        lib.tcsdn_forest_fit_free(h)
+    return classes, dict(a, tree_offsets=offs, n_features=d)
+
+
+def forest_feature_importances(offsets, left, right, feature, impurity, weighted_n_node_samples, d):
+    """RandomForestClassifier.feature_importances_ from the concatenated tree arrays, in scikit-learn's operation order:
+    per tree sk:tree/_tree.pyx Tree.compute_feature_importances (a node-order sum of each split's weighted impurity
+    decrease, then / root weight, then / sum), then the mean over the trees with more than one node
+    (sk:ensemble/_forest.py feature_importances_), divided by its sum."""
+    per_tree = []
+    for t in range(len(offsets) - 1):
+        a, b = int(offsets[t]), int(offsets[t + 1])
+        if b - a <= 1:
+            continue
+        lf, rt, ft = (np.asarray(v[a:b]) for v in (left, right, feature))
+        wn = np.asarray(weighted_n_node_samples[a:b], np.float64)
+        im = np.asarray(impurity[a:b], np.float64)
+        inner = np.flatnonzero(lf != -1)
+        l, r = lf[inner], rt[inner]
+        imp = np.zeros(d, np.float64)
+        np.add.at(imp, ft[inner], wn[inner] * im[inner] - wn[l] * im[l] - wn[r] * im[r])   # unbuffered: node order
+        imp /= wn[0]
+        s = np.sum(imp)
+        if s > 0.0:
+            imp /= s
+        per_tree.append(imp)
+    if not per_tree:
+        return np.zeros(d, np.float64)
+    m = np.mean(per_tree, axis=0, dtype=np.float64)
+    return m / np.sum(m)
+
+
 class RandomForestClassifier(_Base):
     """sk:ensemble/_forest.py:882-967 + sk:tree/_tree.pyx:954-996 -- bit-exact soft vote over the trees."""
     _kind = "forest"
@@ -762,6 +942,21 @@ class RandomForestClassifier(_Base):
         _lib.check(lib.tcsdn_forest_create(_p(offs, _lib._i64p), _p(left, _lib._i32p), _p(right, _lib._i32p),
                                            _p(feat, _lib._i32p), _p(thr, _lib._f64p), _p(val, _lib._f64p),
                                            len(offs) - 1, int(spec["n_features"]), val.shape[1], C.byref(h)))
+
+    def _fit_gpu(self, X, y, strict, node_capacity=0):
+        """RandomForestClassifier.fit on the GPU (forest_fit), only with ``backend="gpu"``: the trees scikit-learn 1.9 grows
+        with the same ``random_state``, node for node and bit for bit.  ``backend="auto"`` keeps scikit-learn on the host."""
+        if not strict:
+            return False
+        classes, a = forest_fit(X, y, self._params, node_capacity)
+        offs, d = a["tree_offsets"], a["n_features"]
+        self._adopt(dict(kind="forest", tree_offsets=offs, left=a["left"], right=a["right"], feature=a["feature"],
+                         threshold=a["threshold"], value=a["value"], classes=classes, n_features=d))
+        self.tree_arrays_ = {k: v for k, v in a.items() if k != "n_features"}
+        self.n_classes_ = len(classes)
+        self.feature_importances_ = forest_feature_importances(offs, a["left"], a["right"], a["feature"], a["impurity"],
+                                                               a["weighted_n_node_samples"], d)
+        return True
 
     def predict_proba(self, X):
         return self._scores(X)
