@@ -259,7 +259,7 @@ int tcsdn_svc_ovr_from_ovo(const double *dec, int64_t n, int32_t n_classes, int3
                            void *cuda_stream);
 
 /* ---- N3 (next row): `.fit` of the two cheap models on the GPU -------------------------------------
- * (RandomForestClassifier has tcsdn_forest_fit below; the other three keep importing fitted parameters from scikit-learn).  X [n][d] float32/float64 and
+ * (RandomForestClassifier and SVC have tcsdn_forest_fit and tcsdn_svc_fit below; the other two keep importing fitted parameters from scikit-learn).  X [n][d] float32/float64 and
  * y / labels_out live where `loc` says; the small outputs (theta, var, ..., centers_out) are HOST arrays.
  * Sums are fp64 and deterministic but not in numpy's order: results agree with scikit-learn to ~1e-13 relative.
  * float32 rows are fitted in fp64 (scikit-learn's fit of the widened rows).  d <= 255.
@@ -328,6 +328,35 @@ int tcsdn_forest_fit_nodes(const tcsdn_forest_fit_t *f, int64_t *tree_offsets);
 int tcsdn_forest_fit_read(const tcsdn_forest_fit_t *f, int32_t *left, int32_t *right, int32_t *feature, double *threshold,
                           double *value, double *impurity, int64_t *n_node_samples, double *weighted_n_node_samples);
 void tcsdn_forest_fit_free(tcsdn_forest_fit_t *f);
+
+/* tcsdn_svc_fit     SVC(kernel in {'linear', 'poly', 'rbf'}, probability=False).fit (sk:svm/_base.py BaseLibSVM.fit,
+ *                   sk:svm/src/libsvm/svm.cpp svm_train, Solver::Solve): the model scikit-learn 1.9.0's libsvm fork
+ *                   computes, bit for bit, iteration for iteration.  One CTA solves one class pair of the one-vs-one loop
+ *                   on the device, with no host round trip per iteration.  X [n][d] float32/float64 lives where `loc`
+ *                   says and is widened to float64 on the device; device rows are never copied to the host.  y [n] (HOST)
+ *                   holds class indices in [0, n_classes), each class at least once.  kernel: 0 linear, 1 poly, 2 rbf
+ *                   (TCSDN_SVC_*; sigmoid is refused).  gamma is the resolved one (scikit-learn's _gamma), class_C
+ *                   [n_classes] (HOST) is C * class_weight_[c], tol is libsvm's eps, max_iter -1 means no limit.
+ *                   1 <= d <= 15 (where scipy's ddot equals an FMA chain in feature order), n < 2^31, C > 0, tol > 0,
+ *                   gamma >= 0, degree >= 0: TCSDN_EINVAL otherwise, before any device work.  TCSDN_ENONFINITE for NaN /
+ *                   inf rows.  A class pair still running after max(10^7, 100 l) iterations (l: its rows) stops and the
+ *                   call returns TCSDN_ECUDA with a message.  The call returns when the model is on the host, in *out.
+ * tcsdn_svc_fit_sizes  *n_sv (support vectors), n_support [n_classes], n_iter [n_classes (n_classes - 1) / 2] and
+ *                   *fit_status (1: max_iter reached in some pair), all HOST.
+ * tcsdn_svc_fit_read   support [n_sv] (row indices), sv [n_sv][d] (those rows, float64), dual_coef [n_classes - 1][n_sv]
+ *                   and intercept [n_classes (n_classes - 1) / 2]: libsvm's sign convention (scikit-learn's _dual_coef_ /
+ *                   _intercept_), HOST arrays.
+ * tcsdn_row_var     X.var() of the n*d values, widened to float64, as numpy computes it (pairwise summation of the mean,
+ *                   then of the squared deviations), for gamma='scale' on rows that stay on the device; device rows are
+ *                   read in place.  *var_out is HOST.  TCSDN_ENONFINITE for NaN / inf rows. */
+typedef struct tcsdn_svc_fit tcsdn_svc_fit_t;
+int tcsdn_svc_fit(const void *x, const int32_t *y, int64_t n, int32_t d, int32_t n_classes, int32_t x_dtype, int32_t loc,
+                  int32_t kernel, double gamma, double coef0, int32_t degree, const double *class_C, double tol,
+                  int32_t shrinking, int64_t max_iter, tcsdn_svc_fit_t **out, void *cuda_stream);
+int tcsdn_svc_fit_sizes(const tcsdn_svc_fit_t *f, int64_t *n_sv, int32_t *n_support, int32_t *n_iter, int32_t *fit_status);
+int tcsdn_svc_fit_read(const tcsdn_svc_fit_t *f, int32_t *support, double *sv, double *dual_coef, double *intercept);
+void tcsdn_svc_fit_free(tcsdn_svc_fit_t *f);
+int tcsdn_row_var(const void *x, int64_t n, int32_t d, int32_t x_dtype, int32_t loc, double *var_out, void *cuda_stream);
 
 /* ---- multi-GPU (SURVEY 8e): one process per GPU, rows sharded, models replicated ------------------
  * predict() never communicates: rank r classifies its contiguous block of n_block = ceil(n / world) rows.  The only

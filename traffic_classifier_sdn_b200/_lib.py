@@ -78,6 +78,12 @@ SIGNATURES = {
     "tcsdn_forest_fit_nodes": (C.c_int, [_vp, _i64p]),
     "tcsdn_forest_fit_read": (C.c_int, [_vp, _i32p, _i32p, _i32p, _f64p, _f64p, _f64p, _i64p, _f64p]),
     "tcsdn_forest_fit_free": (None, [_vp]),
+    "tcsdn_svc_fit": (C.c_int, [_vp, _i32p, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_double,
+                                C.c_double, C.c_int32, _f64p, C.c_double, C.c_int32, C.c_int64, C.POINTER(_vp), _vp]),
+    "tcsdn_svc_fit_sizes": (C.c_int, [_vp, _i64p, _i32p, _i32p, _i32p]),
+    "tcsdn_svc_fit_read": (C.c_int, [_vp, _i32p, _f64p, _f64p, _f64p]),
+    "tcsdn_svc_fit_free": (None, [_vp]),
+    "tcsdn_row_var": (C.c_int, [_vp, C.c_int64, C.c_int32, C.c_int32, C.c_int32, _f64p, _vp]),
     "tcsdn_comm_unique_id": (C.c_int, [_vp]),
     "tcsdn_comm_init": (C.c_int, [C.c_int32, C.c_int32, _vp, C.POINTER(_vp)]),
     "tcsdn_allgather_labels": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, _vp, _vp]),

@@ -8,7 +8,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libtcsdn.so")
-SOURCES = ["abi.cu", "scorers.cu", "forest.cu", "knn.cu", "svc.cu", "flow.cu", "knn_engine.cu", "svc_engine.cu", "comm.cu", "fit.cu", "kmeanspp.cu", "forest_fit.cu"]
+SOURCES = ["abi.cu", "scorers.cu", "forest.cu", "knn.cu", "svc.cu", "flow.cu", "knn_engine.cu", "svc_engine.cu", "comm.cu", "fit.cu", "kmeanspp.cu", "forest_fit.cu", "svc_fit.cu"]
 # scorers.cu is compiled five times: once as the dispatcher and once per tiled feature count (object name -> extra flags)
 VARIANTS = {"scorers.cu": [("scorers.o", []), ("scorers_d4.o", ["-DTCSDN_SCORER_D=4"]), ("scorers_d8.o", ["-DTCSDN_SCORER_D=8"]),
                            ("scorers_d12.o", ["-DTCSDN_SCORER_D=12"]), ("scorers_d16.o", ["-DTCSDN_SCORER_D=16"])]}

@@ -98,8 +98,9 @@ class _Base:
 
     def fit(self, X, y=None, backend="auto"):
         """Train, then move the fitted parameters to HBM.  GaussianNB and KMeans fit on the GPU (SURVEY row N3,
-        csrc/fit.cu) unless ``backend="sklearn"``; RandomForestClassifier fits on the GPU with ``backend="gpu"``
-        (csrc/forest_fit.cu) and with scikit-learn on the host otherwise; the other three train with scikit-learn."""
+        csrc/fit.cu) unless ``backend="sklearn"``; RandomForestClassifier and SVC fit on the GPU with ``backend="gpu"``
+        (csrc/forest_fit.cu, csrc/svc_fit.cu) and with scikit-learn on the host otherwise; LogisticRegression and
+        KNeighborsClassifier train with scikit-learn."""
         if backend not in ("auto", "gpu", "sklearn"):
             raise ValueError("backend must be 'auto', 'gpu' or 'sklearn'")
         if backend != "sklearn" and self._fit_gpu(X, y, strict=backend == "gpu"):
@@ -742,6 +743,158 @@ class SVC(_Base):
         if self.break_ties and self.decision_function_shape == "ovr" and len(self.classes_) > 2:
             return self.classes_.take(np.argmax(self.decision_function(X), axis=1))  # sk:svm/_base.py:851-858
         return super().predict(X)
+
+    def _fit_gpu(self, X, y, strict):
+        """SVC.fit on the GPU (svc_fit), only with ``backend="gpu"``: scikit-learn 1.9.0's fitted model, bit for bit.
+        ``backend="auto"`` keeps scikit-learn on the host."""
+        if not strict:
+            return False
+        m = svc_fit(X, y, self._params)
+        self._adopt(dict(kind="svc", sv=m["support_vectors_"], dual_coef=m["_dual_coef_"], intercept=m["_intercept_"],
+                         n_support=m["n_support_"], gamma=m["_gamma"], classes=m["classes_"], n_features=m["shape_fit_"][1],
+                         decision_function_shape=str(self._params.get("decision_function_shape", "ovr")),
+                         break_ties=bool(self._params.get("break_ties", False)), n_classes=len(m["classes_"]),
+                         kernel=m["kernel"], coef0=m["coef0"], degree=m["degree"]))
+        for k in ("support_", "dual_coef_", "intercept_", "_dual_coef_", "_intercept_", "n_iter_", "fit_status_",
+                  "class_weight_", "shape_fit_"):
+            setattr(self, k, m[k])
+        return True
+
+
+_SVC_GPU_PARAMS = ("C", "kernel", "degree", "gamma", "coef0", "shrinking", "probability", "tol", "cache_size",
+                   "class_weight", "verbose", "max_iter", "decision_function_shape", "break_ties", "random_state")
+SVC_FIT_MAX_FEATURES = 15
+
+
+def _real(v):
+    import numbers
+    return isinstance(v, numbers.Real) and not isinstance(v, bool)
+
+
+def svc_fit_plan(params, X, y):
+    """Host half of SVC.fit (sk:svm/_base.py BaseLibSVM.fit and BaseSVC._validate_targets) for the GPU fit: -> dict with
+    ``classes_``, ``y_index`` (int32 class index per row), ``class_weight_``, ``class_C`` (C * class_weight_),
+    ``_gamma``, ``kernel``, ``degree``, ``coef0``, ``tol``, ``shrinking`` and ``max_iter``.  X: numpy rows or a CUDA
+    tensor (gamma='scale' then takes numpy's X.var() on the device, tcsdn_row_var); y: labels on the host or the device.
+    Raises ValueError naming what the GPU fit does not support: probability=True, kernel 'sigmoid' / 'precomputed' /
+    callable, 16 or more features, NaN / inf host rows, lengths that differ, a single class."""
+    import numbers
+    from sklearn.utils.class_weight import compute_class_weight
+    p = dict(params)
+    for k in p:
+        if k not in _SVC_GPU_PARAMS:
+            raise ValueError(f"SVC GPU fit: unknown parameter {k}")
+    prob = p.get("probability", "deprecated")
+    if prob is True:
+        raise ValueError("SVC GPU fit: probability=True is not supported (Platt scaling needs libsvm's internal "
+                         "cross-validation); fit with backend='sklearn'")
+    kernel = p.get("kernel", "rbf")
+    if callable(kernel) or not isinstance(kernel, str) or kernel not in ("linear", "poly", "rbf"):
+        raise ValueError(f"SVC GPU fit: kernel={kernel!r} is not supported (kernel must be 'linear', 'poly' or 'rbf')")
+    Cv = p.get("C", 1.0)
+    if not _real(Cv) or not 0.0 < Cv < np.inf:
+        raise ValueError(f"C must be a float > 0, got {Cv!r}")
+    degree = p.get("degree", 3)
+    if not isinstance(degree, numbers.Integral) or isinstance(degree, bool) or not 0 <= degree < 2 ** 31:
+        raise ValueError(f"degree must be an integer >= 0, got {degree!r}")
+    coef0 = p.get("coef0", 0.0)
+    if not _real(coef0) or not np.isfinite(coef0):
+        raise ValueError(f"coef0 must be a finite float, got {coef0!r}")
+    tol = p.get("tol", 1e-3)
+    if not _real(tol) or not 0.0 < tol < np.inf:
+        raise ValueError(f"tol must be a float > 0, got {tol!r}")
+    max_iter = p.get("max_iter", -1)
+    if not isinstance(max_iter, numbers.Integral) or isinstance(max_iter, bool) or max_iter < -1:
+        raise ValueError(f"max_iter must be an integer >= -1, got {max_iter!r}")
+    shrinking = p.get("shrinking", True)
+    if not isinstance(shrinking, (bool, np.bool_)):
+        raise ValueError(f"shrinking must be a bool, got {shrinking!r}")
+    gamma = p.get("gamma", "scale")
+    if not (gamma in ("scale", "auto") if isinstance(gamma, str) else _real(gamma) and 0.0 <= gamma < np.inf):
+        raise ValueError(f"gamma must be 'scale', 'auto' or a float >= 0, got {gamma!r}")
+    ptr, n, d, dt, loc, keep = _Base._fit_rows(X)
+    if d > SVC_FIT_MAX_FEATURES:
+        raise ValueError(f"SVC GPU fit: X has {d} features; the GPU fit supports at most {SVC_FIT_MAX_FEATURES} "
+                         "(n_features_in_ <= 15, where libsvm's BLAS dot is an FMA chain in feature order)")
+    if loc == _lib.HOST and not np.isfinite(keep).all():
+        raise ValueError("Input X contains NaN or infinity.")
+    if y is None:
+        raise ValueError("SVC.fit needs y")
+    if _is_torch_cuda(y):
+        y = y.cpu().numpy()
+    y = np.asarray(y)
+    if y.ndim != 1:
+        y = y.ravel() if y.ndim == 2 and y.shape[1] == 1 else y
+    if y.ndim != 1:
+        raise ValueError(f"y should be a 1d array, got an array of shape {y.shape} instead.")
+    if len(y) != n:
+        raise ValueError(f"Found input variables with inconsistent numbers of samples: [{n}, {len(y)}]")
+    if n >= 2 ** 31:
+        raise ValueError(f"the GPU fit supports fewer than 2^31 rows (got {n})")
+    classes, yi = np.unique(y, return_inverse=True)
+    class_weight = compute_class_weight(p.get("class_weight"), classes=classes, y=y)
+    if len(classes) < 2:
+        raise ValueError("The number of classes has to be greater than one; got %d class" % len(classes))
+    if isinstance(gamma, str) and gamma == "scale":
+        if loc == _lib.HOST:
+            var = np.asarray(keep, dtype=np.float64).var()
+        else:
+            v = C.c_double()
+            import torch
+            _lib.check(_lib.load().tcsdn_row_var(ptr, n, d, dt, loc, C.byref(v), torch.cuda.current_stream(keep.device).cuda_stream))
+            var = np.float64(v.value)
+        g = 1.0 / (d * var) if var != 0 else 1.0
+    elif isinstance(gamma, str):
+        g = 1.0 / d
+    else:
+        g = gamma
+    class_C = np.ascontiguousarray(np.asarray(class_weight, np.float64) * float(Cv))   # libsvm: weighted_C = C * weight
+    if not (np.isfinite(class_C).all() and (class_C > 0).all()):
+        raise ValueError(f"class_weight: every class needs a weight > 0 for the GPU fit, got {class_weight!r}")
+    return dict(classes_=classes, y_index=np.ascontiguousarray(yi.ravel(), np.int32), class_weight_=class_weight,
+                class_C=class_C, _gamma=g, kernel=kernel, degree=int(degree), coef0=float(coef0), tol=float(tol),
+                shrinking=bool(shrinking), max_iter=int(max_iter), rows=(ptr, n, d, dt, loc, keep))
+
+
+def svc_fit(X, y, params):
+    """SVC(**params).fit(X, y) on the GPU (tcsdn_svc_fit): -> dict of scikit-learn's fitted attributes (``support_``,
+    ``support_vectors_``, ``n_support_``, ``dual_coef_``, ``intercept_``, ``_dual_coef_``, ``_intercept_``, ``n_iter_``,
+    ``fit_status_``, ``class_weight_``, ``_gamma``, ``classes_``, ``shape_fit_``) plus ``kernel``, ``coef0`` and
+    ``degree``.  Raises scikit-learn's ConvergenceWarning when max_iter stopped a class pair."""
+    import warnings
+    plan = svc_fit_plan(params, X, y)
+    ptr, n, d, dt, loc, keep = plan.pop("rows")
+    classes = plan["classes_"]
+    Cn, lib = len(classes), _lib.load()
+    P = Cn * (Cn - 1) // 2
+    st = None
+    if loc == _lib.DEVICE:
+        import torch
+        st = torch.cuda.current_stream(keep.device).cuda_stream
+    h = C.c_void_p()
+    _lib.check(lib.tcsdn_svc_fit(ptr, _p(plan["y_index"], _lib._i32p), n, d, Cn, dt, loc, _lib.SVC_KERNELS[plan["kernel"]],
+                                 float(plan["_gamma"]), plan["coef0"], plan["degree"], _p(plan["class_C"], _lib._f64p),
+                                 plan["tol"], int(plan["shrinking"]), plan["max_iter"], C.byref(h), st))
+    try:
+        n_sv, status = C.c_int64(), C.c_int32()
+        nsup, n_iter = np.empty(Cn, np.int32), np.empty(P, np.intc)
+        _lib.check(lib.tcsdn_svc_fit_sizes(h, C.byref(n_sv), _p(nsup, _lib._i32p), _p(n_iter, _lib._i32p), C.byref(status)))
+        m = int(n_sv.value)
+        support, sv = np.empty(m, np.int32), np.empty((m, d), np.float64)
+        dual, icpt = np.empty((Cn - 1, m), np.float64), np.empty(P, np.float64)
+        _lib.check(lib.tcsdn_svc_fit_read(h, _p(support, _lib._i32p), _p(sv, _lib._f64p), _p(dual, _lib._f64p),
+                                          _p(icpt, _lib._f64p)))
+    finally:
+        lib.tcsdn_svc_fit_free(h)
+    out = dict(support_=support, support_vectors_=sv, n_support_=nsup, _dual_coef_=dual, _intercept_=icpt,
+               dual_coef_=-dual if Cn == 2 else dual, intercept_=-icpt if Cn == 2 else icpt.copy(), n_iter_=n_iter,
+               fit_status_=int(status.value), class_weight_=plan["class_weight_"], _gamma=plan["_gamma"], classes_=classes,
+               shape_fit_=(n, d), kernel=plan["kernel"], coef0=plan["coef0"], degree=plan["degree"])
+    if out["fit_status_"] == 1:   # sk:svm/_base.py _warn_from_fit_status
+        from sklearn.exceptions import ConvergenceWarning
+        warnings.warn("Solver terminated early (max_iter=%i).  Consider pre-processing your data with StandardScaler "
+                      "or MinMaxScaler." % plan["max_iter"], ConvergenceWarning)
+    return out
 
 
 _FOREST_GPU_PARAMS = ("n_estimators", "criterion", "max_depth", "min_samples_split", "min_samples_leaf", "max_features",
